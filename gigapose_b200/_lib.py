@@ -39,6 +39,21 @@ class GpMatches(C.Structure):
                 ("src_pts", C.c_void_p)]
 
 
+class GpDebugGemm(C.Structure):
+    _fields_ = [("M", C.c_int32), ("N", C.c_int32), ("K", C.c_int32), ("bn", C.c_int32), ("passes", C.c_int32),
+                ("mode", C.c_int32), ("swap", C.c_int32), ("f16", C.c_int32), ("acc_scale", C.c_float),
+                ("a_hi", C.c_void_p), ("a_lo", C.c_void_p), ("w_hi", C.c_void_p), ("w_lo", C.c_void_p),
+                ("out_hi", C.c_void_p), ("out_lo", C.c_void_p), ("bias", C.c_void_p), ("gamma", C.c_void_p),
+                ("x", C.c_void_p), ("pos", C.c_void_p), ("res_hi", C.c_void_p), ("res_lo", C.c_void_p),
+                ("m_dev", C.c_void_p), ("tokens_per_img", C.c_int32), ("patches_per_img", C.c_int32),
+                ("qkv_crop_stride", C.c_int32)]
+
+
+# gp_debug_gemm_t.mode
+GEMM_PLANES, GEMM_PLANES_GELU, GEMM_SCALE_RESIDUAL, GEMM_PATCH_EMBED, GEMM_QKV_HEADS = 0, 1, 2, 3, 4
+GEMM_PLANES_RELU, GEMM_PLANES_ADD_RELU, GEMM_ROWS_F32, GEMM_ROWS_F32_RELU = 5, 6, 7, 8
+
+
 class GpRansacOut(C.Structure):
     _fields_ = [("M", C.c_void_p), ("failed", C.c_void_p), ("inlier_src_pts", C.c_void_p),
                 ("inlier_tar_pts", C.c_void_p), ("inlier_scores", C.c_void_p), ("inlier_count", C.c_void_p)]
@@ -96,6 +111,9 @@ SYMBOLS = {
     "gp_ist_trunk_forward": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
     "gp_debug_ist_trunk": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
     "gp_debug_sim_tiles": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
+    "gp_debug_gemm": (C.c_int, [C.POINTER(GpDebugGemm), C.c_void_p]),
+    "gp_debug_attention": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                     C.c_void_p]),
     "gp_normalize_patch_tokens": (C.c_int, [C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
     "gp_vit_time_linears": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.POINTER(C.c_float), C.c_void_p]),
     "gp_time_sim_kernel": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.POINTER(C.c_float), C.c_void_p]),

@@ -237,6 +237,7 @@ int validate(const gp_config_t* cfg) {
   if (cfg->num_templates_global < cfg->top_k) return fail(GP_ERR_INVALID, "fewer templates than top_k (torch.topk would raise)");
   if (cfg->template_id_stride < 1 || cfg->template_id_offset < 0) return fail(GP_ERR_INVALID, "bad template id stride/offset");
   if (cfg->patch_size < 1) return fail(GP_ERR_INVALID, "patch_size must be >= 1");
+  if (cfg->sim_threshold != cfg->sim_threshold) return fail(GP_ERR_INVALID, "sim_threshold is NaN");
   if (cfg->precision != GP_PRECISION_FP32_SPLIT && cfg->precision != GP_PRECISION_BF16)
     return fail(GP_ERR_INVALID, "unknown precision %d", cfg->precision);
   if (cfg->ist_bank_global != 0 && cfg->ist_bank_global != 1) return fail(GP_ERR_INVALID, "ist_bank_global must be 0 or 1");

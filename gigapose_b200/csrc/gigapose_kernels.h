@@ -200,7 +200,7 @@ struct GemmParams {
   const float* pos;           // [257,N] positional table (GEMM_PATCH_EMBED)
   int tokens_per_img, patches_per_img;
   int qkv_crop_stride;        // GEMM_QKV_HEADS: crops per q/k/v section of the head-major planes (= max_crops)
-  int bn;                     // output-tile width: 128, 192 or 256 (0 = 256); N % bn == 0
+  int bn;                     // output-tile width: 192 or 256 (0 = 256); N % bn == 0
   // implicit-GEMM convolution (conv != 0): A is an NHWC plane read through a 4-D tensor map, one k-block per
   // (filter tap, 32-channel block); a 128-row tile is 128 / Wo whole output rows of one image
   int conv, Ho, Wo, stride, pad, kw, cblocks;
@@ -212,6 +212,9 @@ struct GemmParams {
   int f16;                    // operand (and output) planes hold IEEE fp16 hi/lo pairs instead of bf16: 22 significant bits
                               // for O(1)-range data (the IST MLP), wgmma with fp16 A/B formats
 };
+// whether vit_gemm_kernel has an instantiation for p's (swap, bn, f16, mode) and p's shape tiles; `why` (nullable)
+// receives the reason when it does not.  Host-only: needs no device.
+bool gemm_config_supported(const GemmParams& p, const char** why = nullptr);
 cudaError_t launch_vit_gemm(const CUtensorMap& a_hi, const CUtensorMap& a_lo, const CUtensorMap& w_hi,
                             const CUtensorMap& w_lo, const GemmParams& p, int num_sms, cudaStream_t stream);
 cudaError_t launch_split_planes(const float* x, long long rows, int K, int Kpad, uint16_t* hi, uint16_t* lo, cudaStream_t s,

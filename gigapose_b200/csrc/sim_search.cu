@@ -54,7 +54,7 @@ __device__ __forceinline__ void decode_item(int item, int B, int T, int& j, int&
 }
 
 struct __align__(8) SimSmemTail {
-  unsigned long long colkey[kP];                // per column s: max over t of (bits(v) << 32 | 255 - t)
+  unsigned long long colkey[kP];                // per column s: max over t of (ord(v) << 32 | 255 - t)
   float smask[kP];                              // template mask sampled at 16x16 (float: alpha masks are not binary)
   float tmask[kP];                              // query mask sampled at 16x16
   float cmax[kP];                               // score_src2tar
@@ -72,7 +72,10 @@ constexpr int kSmemBytes = 1024 /*alignment slack*/ + kStages * kStageBytes + si
 
 // Work unit of the producer: (item, t-half) = a 128(t) x 256(s) x 1024(c) half tile; the template planes are streamed
 // once per half.
-template <bool kDebug>
+// kSigned: sim_threshold <= 0 lets negative values (and -0.0 from masked patches) through the threshold.  The column
+// arg-max key then maps the float to an order-preserving uint32 (-0.0 folded into +0.0) instead of taking its bits as
+// they are, which orders only values >= +0.0; the row maximum starts at -inf instead of -1.
+template <bool kDebug, bool kSigned>
 __global__ void __launch_bounds__(kThreads, 1)
 sim_search_kernel(const __grid_constant__ CUtensorMap tm_q_hi, const __grid_constant__ CUtensorMap tm_q_lo,
                   const __grid_constant__ CUtensorMap tm_t_hi, const __grid_constant__ CUtensorMap tm_t_lo,
@@ -190,7 +193,8 @@ sim_search_kernel(const __grid_constant__ CUtensorMap tm_q_hi, const __grid_cons
         // accumulator fragment: rows t0 = .. + lane/4 and t0 + 8, columns s = 8 j8 + 2 (lane % 4) + {0, 1}
         const int t0 = half * kHalfRows + wg * 64 + wl * 16 + (lane >> 2), t1 = t0 + 8;
         const float tm0 = tail.tmask[t0], tm1 = tail.tmask[t1];
-        float rbest0 = -1.0f, rbest1 = -1.0f;  // all candidates are >= 0 after thresholding -> first max wins
+        // thr > 0: all candidates are >= 0 after thresholding -> first max wins
+        float rbest0 = kSigned ? -INFINITY : -1.0f, rbest1 = kSigned ? -INFINITY : -1.0f;
         int ridx0 = 0, ridx1 = 0;
 #pragma unroll
         for (int j8 = 0; j8 < kP / 8; ++j8) {
@@ -199,8 +203,9 @@ sim_search_kernel(const __grid_constant__ CUtensorMap tm_q_hi, const __grid_cons
             const int s = 8 * j8 + 2 * (lane & 3) + c;
             const float raw0 = acc[4 * j8 + c], raw1 = acc[4 * j8 + 2 + c];
             if (kDebug) {
-              p.debug_tile[((size_t)item * kP + t0) * kP + s] = raw0;
-              p.debug_tile[((size_t)item * kP + t1) * kP + s] = raw1;
+              const size_t tile = (size_t)n * p.B + j;
+              p.debug_tile[(tile * kP + t0) * kP + s] = raw0;
+              p.debug_tile[(tile * kP + t1) * kP + s] = raw1;
             }
             const float sm = tail.smask[s];
             float v0 = raw0 * sm, v1 = raw1 * sm;                             // matching.py:234
@@ -210,7 +215,11 @@ sim_search_kernel(const __grid_constant__ CUtensorMap tm_q_hi, const __grid_cons
             if (v1 > rbest1) { rbest1 = v1; ridx1 = s; }
             // torch.max(dim=2): first maximum over t.  v >= 0: float order == uint order; ties -> the smaller t
             const bool second = v1 > v0;
-            const uint32_t bits = __float_as_uint(second ? v1 : v0);
+            uint32_t bits = __float_as_uint(second ? v1 : v0);
+            if constexpr (kSigned) {
+              bits = bits == 0x80000000u ? 0u : bits;                         // -0.0 == +0.0 for torch.max
+              bits ^= (uint32_t)((int)bits >> 31) | 0x80000000u;              // order-preserving float -> uint32
+            }
             const unsigned long long key = ((unsigned long long)bits << 32) | (unsigned)(255 - (second ? t1 : t0));
             atomicMax(&tail.colkey[s], key);
           }
@@ -231,7 +240,9 @@ sim_search_kernel(const __grid_constant__ CUtensorMap tm_q_hi, const __grid_cons
       named_barrier_sync(1, kEpiThreads);
       {
         const unsigned long long key = tail.colkey[tid];
-        tail.cmax[tid] = __uint_as_float((uint32_t)(key >> 32));
+        uint32_t bits = (uint32_t)(key >> 32);
+        if constexpr (kSigned) bits = (bits & 0x80000000u) ? (bits ^ 0x80000000u) : ~bits;
+        tail.cmax[tid] = __uint_as_float(bits);
         tail.cidx[tid] = (uint8_t)(255u - (uint32_t)(key & 0xffu));
       }
       named_barrier_sync(1, kEpiThreads);
@@ -311,7 +322,7 @@ topk_select_kernel(TopkSelectParams p) {
       if (bi < p.T) {
         p.cand_score[o] = bv;
         p.cand_id[o] = bi * p.id_stride + p.id_offset;
-        s_val[bi] = -INFINITY;                     // exclude from later rounds (scores themselves are >= 0)
+        s_val[bi] = -INFINITY;                     // exclude from later rounds (no score is -inf: they are finite)
       } else {                                     // fewer than k local templates: padding candidate
         p.cand_score[o] = -INFINITY;
         p.cand_id[o] = 0x7fffffff;
@@ -403,17 +414,19 @@ cudaError_t launch_sim_search(const CUtensorMap& q_hi, const CUtensorMap& q_lo, 
                               const CUtensorMap& t_lo, const SimSearchParams& p, int num_sms, cudaStream_t stream) {
   static bool configured = false;
   if (!configured) {
-    cudaError_t e = cudaFuncSetAttribute(sim_search_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes);
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(sim_search_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes);
+    cudaError_t e = cudaSuccess;
+    for (auto k : {sim_search_kernel<false, false>, sim_search_kernel<true, false>, sim_search_kernel<false, true>,
+                   sim_search_kernel<true, true>})
+      if (e == cudaSuccess) e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes);
     if (e != cudaSuccess) return e;
     configured = true;
   }
   if (p.num_items <= 0) return cudaSuccess;
   const int grid = p.num_items < num_sms ? p.num_items : num_sms;
-  if (p.debug_tile)
-    sim_search_kernel<true><<<grid, kThreads, kSmemBytes, stream>>>(q_hi, q_lo, t_hi, t_lo, p);
-  else
-    sim_search_kernel<false><<<grid, kThreads, kSmemBytes, stream>>>(q_hi, q_lo, t_hi, t_lo, p);
+  const bool sign = !(p.sim_threshold > 0.f);         // negative values survive the threshold
+  auto kernel = p.debug_tile ? (sign ? sim_search_kernel<true, true> : sim_search_kernel<true, false>)
+                             : (sign ? sim_search_kernel<false, true> : sim_search_kernel<false, false>);
+  kernel<<<grid, kThreads, kSmemBytes, stream>>>(q_hi, q_lo, t_hi, t_lo, p);
   return cudaGetLastError();
 }
 

@@ -175,6 +175,63 @@ int gp_debug_gemm_timeline(long long* stamps64) {
   return GP_OK;
 }
 
+int gp_debug_gemm(const gp_debug_gemm_t* d, void* stream) {
+  if (!d) return gp_internal_fail(GP_ERR_INVALID, "null argument");
+  gp::GemmParams g{};
+  g.M = d->M; g.N = d->N; g.K = d->K; g.bn = d->bn; g.passes = d->passes; g.mode = d->mode; g.swap = d->swap; g.f16 = d->f16;
+  g.acc_scale = d->acc_scale; g.bias = d->bias; g.gamma = d->gamma; g.x = d->x; g.out_hi = d->out_hi; g.out_lo = d->out_lo;
+  g.pos = d->pos; g.res_hi = d->res_hi; g.res_lo = d->res_lo; g.m_dev = d->m_dev;
+  g.tokens_per_img = d->tokens_per_img; g.patches_per_img = d->patches_per_img; g.qkv_crop_stride = d->qkv_crop_stride;
+  if (g.M < 1) return gp_internal_fail(GP_ERR_INVALID, "M must be >= 1");
+  const char* why = nullptr;
+  if (!gp::gemm_config_supported(g, &why)) return gp_internal_fail(GP_ERR_INVALID, "unsupported GEMM: %s", why);
+  if (!d->a_hi || !d->a_lo || !d->w_hi || !d->w_lo || !d->bias) return gp_internal_fail(GP_ERR_INVALID, "null operand or bias");
+  const bool planes_out = g.mode == gp::GEMM_PLANES || g.mode == gp::GEMM_PLANES_GELU || g.mode == gp::GEMM_QKV_HEADS ||
+                          g.mode == gp::GEMM_PLANES_RELU || g.mode == gp::GEMM_PLANES_ADD_RELU;
+  if (planes_out ? (!g.out_hi || !g.out_lo) : !g.x) return gp_internal_fail(GP_ERR_INVALID, "null output");
+  if (g.mode == gp::GEMM_SCALE_RESIDUAL && !g.gamma) return gp_internal_fail(GP_ERR_INVALID, "null gamma");
+  if (g.mode == gp::GEMM_PLANES_ADD_RELU && (!g.res_hi || !g.res_lo)) return gp_internal_fail(GP_ERR_INVALID, "null residual planes");
+  if (g.mode == gp::GEMM_PATCH_EMBED && (!g.pos || g.patches_per_img < 1 || g.tokens_per_img <= g.patches_per_img))
+    return gp_internal_fail(GP_ERR_INVALID, "patch embedding needs pos and tokens_per_img > patches_per_img >= 1");
+  if (g.mode == gp::GEMM_QKV_HEADS && (g.N != kQkv || g.tokens_per_img < 1 || g.qkv_crop_stride * g.tokens_per_img < g.M))
+    return gp_internal_fail(GP_ERR_INVALID, "QKV scatter needs N = 3072 and qkv_crop_stride * tokens_per_img >= M");
+  if (g.swap && g.m_dev) return gp_internal_fail(GP_ERR_INVALID, "m_dev is not supported with swap");
+  int dev = 0, sms = 0;
+  GPV_CUDA(cudaGetDevice(&dev));
+  GPV_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+  const int bn = g.bn > 0 ? g.bn : 256;
+  // A: 128-row boxes; W: bn-row boxes (the swapped form streams 256 output pixels as its W operand)
+  CUtensorMap a_hi, a_lo, w_hi, w_lo;
+  auto* a_h = const_cast<uint16_t*>(d->a_hi); auto* a_l = const_cast<uint16_t*>(d->a_lo);
+  auto* w_h = const_cast<uint16_t*>(d->w_hi); auto* w_l = const_cast<uint16_t*>(d->w_lo);
+  if (int e = gp_internal_make_map(&a_hi, a_h, g.M, g.K, 128)) return e;
+  if (int e = gp_internal_make_map(&a_lo, a_l, g.M, g.K, 128)) return e;
+  if (int e = gp_internal_make_map(&w_hi, w_h, g.N, g.K, bn)) return e;
+  if (int e = gp_internal_make_map(&w_lo, w_l, g.N, g.K, bn)) return e;
+  GPV_CUDA(gp::launch_vit_gemm(a_hi, a_lo, w_hi, w_lo, g, sms, static_cast<cudaStream_t>(stream)));
+  gp_internal_count_launches(1);
+  return GP_OK;
+}
+
+int gp_debug_attention(int b, int crop_stride, int passes, const uint16_t* qkv_hi, const uint16_t* qkv_lo, uint16_t* out_hi,
+                       uint16_t* out_lo, void* stream) {
+  if (!qkv_hi || !qkv_lo || !out_hi || !out_lo) return gp_internal_fail(GP_ERR_INVALID, "null argument");
+  if (b < 1 || crop_stride < b) return gp_internal_fail(GP_ERR_INVALID, "need 1 <= b (%d) <= crop_stride (%d)", b, crop_stride);
+  if (passes != 1 && passes != 3) return gp_internal_fail(GP_ERR_INVALID, "passes must be 1 or 3");
+  // the same four maps as gp_vit_create: 64 columns x {128, 16} token rows over all 3 * crop_stride * 16 heads
+  const uint64_t rows = 48ull * crop_stride * kTok;
+  auto* qh = const_cast<uint16_t*>(qkv_hi); auto* ql = const_cast<uint16_t*>(qkv_lo);
+  CUtensorMap hi128, lo128, hi16, lo16;
+  if (int e = gp_internal_make_map_ex(&hi128, qh, rows, 64, 64, 128, 128)) return e;
+  if (int e = gp_internal_make_map_ex(&lo128, ql, rows, 64, 64, 128, 128)) return e;
+  if (int e = gp_internal_make_map_ex(&hi16, qh, rows, 64, 64, 16, 128)) return e;
+  if (int e = gp_internal_make_map_ex(&lo16, ql, rows, 64, 64, 16, 128)) return e;
+  GPV_CUDA(gp::launch_attention_tc(hi128, lo128, hi16, lo16, qkv_hi, qkv_lo, out_hi, out_lo, b, crop_stride, passes,
+                                   static_cast<cudaStream_t>(stream)));
+  gp_internal_count_launches(1);
+  return GP_OK;
+}
+
 int gp_vit_destroy(gp_vit_handle_t h) {
   delete h;
   return GP_OK;

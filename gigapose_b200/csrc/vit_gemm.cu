@@ -102,7 +102,6 @@ __device__ __forceinline__ void gemm_kblock(float (&d)[kN / 2], uint32_t a_hi, u
         const uint32_t accum = (!first || pass != 0 || k16 != 0) ? 1u : 0u;
         if constexpr (kN == 256) { if constexpr (kF16) wgmma_ss_n256_f16(d, da, dw, accum); else wgmma_ss_n256_bf16(d, da, dw, accum); }
         if constexpr (kN == 192) { if constexpr (kF16) wgmma_ss_n192_f16(d, da, dw, accum); else wgmma_ss_n192_bf16(d, da, dw, accum); }
-        if constexpr (kN == 128) { if constexpr (kF16) wgmma_ss_n128_f16(d, da, dw, accum); else wgmma_ss_n128_bf16(d, da, dw, accum); }
       }
     }
   }
@@ -115,7 +114,7 @@ __device__ __forceinline__ void gemm_kblock(float (&d)[kN / 2], uint32_t a_hi, u
 // bank [128, K] and the 256-row operand is a tile of 256 output pixels, so that the tensor pipe still runs N = 256
 // instructions (an N = 128 instruction re-reads its A operand from shared memory twice as often per FLOP); the epilogue
 // transposes the [channel, pixel] accumulator back to NHWC.
-// kTileN (128 / 192 / 256 output columns per tile) and kF16 (operand planes hold fp16 instead of bf16 pairs) are
+// kTileN (192 / 256 output columns per tile) and kF16 (operand planes hold fp16 instead of bf16 pairs) are
 // template parameters too: a runtime choice inside the k-loop makes ptxas insert warpgroup waits between the MMAs.
 template <bool kSwap, int kTileN, bool kF16, int kMode>
 __global__ void __launch_bounds__(kThreads, 1)
@@ -247,7 +246,7 @@ vit_gemm_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_consta
       // ---------------- epilogue: thread = row r, columns [ch * bn/2, (ch + 1) * bn/2) in chunks of 32
       const uint32_t acc = acc_i;
       const int m = mt * kBM + r;
-      const int half_cols = bn >> 1;                   // columns per epilogue warp: 64 / 96 / 128
+      const int half_cols = bn >> 1;                   // columns per epilogue warp: 96 / 128
       const int n0 = ntile0 + ch * half_cols;
       const float* sb = tail.bias_s[acc] + ch * half_cols;
       const float* sg = tail.gamma_s[acc] + ch * half_cols;
@@ -461,19 +460,35 @@ cudaError_t launch_mode(const CUtensorMap& a_hi, const CUtensorMap& a_lo, const 
 }
 }  // namespace
 
-// Instantiated combinations: every mode at 256 columns (bf16); the three bf16-plane modes also at 192 / 128 columns and
-// with the filters as the 128-row operand (kSwap, 256 columns); fp16 pairs for the two regressor layers.  Anything else
-// is rejected with cudaErrorInvalidValue.
+// Instantiated combinations: every mode at 256 columns (bf16); the three bf16-plane modes also at 192 columns and with
+// the filters as the 128-row operand (kSwap, 256 columns); fp16 pairs for the two regressor layers.
+bool gemm_config_supported(const GemmParams& p, const char** why) {
+  if (why) *why = nullptr;
+  auto no = [&](const char* msg) { if (why) *why = msg; return false; };
+  const int bn = p.bn > 0 ? p.bn : kBN;
+  const bool plane_mode = p.mode == GEMM_PLANES || p.mode == GEMM_PLANES_RELU || p.mode == GEMM_PLANES_ADD_RELU;
+  if (bn != 192 && bn != 256) return no("bn must be 192 or 256 (0 = 256)");
+  if (p.N <= 0 || p.N % bn != 0) return no("N must be a positive multiple of bn");
+  if (p.K <= 0 || p.K % kBlockK != 0) return no("K must be a positive multiple of 32");
+  if (p.passes != 1 && p.passes != 3) return no("passes must be 1 or 3");
+  if (p.mode < GEMM_PLANES || p.mode > GEMM_ROWS_F32_RELU) return no("unknown mode");
+  const int tile_pixels = p.swap ? bn : kBM;
+  if (p.conv && (p.Wo <= 0 || tile_pixels % p.Wo != 0 || p.M % kBM != 0 || p.cblocks <= 0))
+    return no("convolution geometry does not tile");
+  if (p.swap && (bn != kBN || p.M % kBM != 0 || p.f16 || !plane_mode))
+    return no("swap needs bn = 256, M % 128 == 0, bf16 planes and a plane mode without GELU");
+  if (p.f16 && (bn != kBN || (p.mode != GEMM_PLANES_RELU && p.mode != GEMM_ROWS_F32_RELU)))
+    return no("f16 needs bn = 256 and mode PLANES_RELU or ROWS_F32_RELU");
+  if (bn == 192 && !plane_mode) return no("bn = 192 supports the modes PLANES, PLANES_RELU and PLANES_ADD_RELU only");
+  return true;
+}
+
+// Anything gemm_config_supported() rejects returns cudaErrorInvalidValue.
 cudaError_t launch_vit_gemm(const CUtensorMap& a_hi, const CUtensorMap& a_lo, const CUtensorMap& w_hi,
                             const CUtensorMap& w_lo, const GemmParams& p, int num_sms, cudaStream_t stream) {
   if (p.M <= 0) return cudaSuccess;
+  if (!gemm_config_supported(p)) return cudaErrorInvalidValue;
   const int bn = p.bn > 0 ? p.bn : kBN;
-  if ((bn != 128 && bn != 192 && bn != 256) || p.N % bn != 0 || p.K % kBlockK != 0) return cudaErrorInvalidValue;
-  const int tile_pixels = p.swap ? bn : kBM;
-  if (p.conv && (p.Wo <= 0 || tile_pixels % p.Wo != 0 || p.M % kBM != 0 || p.cblocks <= 0)) return cudaErrorInvalidValue;
-  if (p.swap && (bn != kBN || p.M % kBM != 0 || p.f16 ||
-                 (p.mode != GEMM_PLANES && p.mode != GEMM_PLANES_RELU && p.mode != GEMM_PLANES_ADD_RELU)))
-    return cudaErrorInvalidValue;
   const int tiles = ((p.M + kBM - 1) / kBM) * (p.N / bn);
   const int grid = tiles < num_sms ? tiles : num_sms;
 #define GP_GEMM_CASE(SWAP, N, F16, MODE) \
@@ -487,7 +502,6 @@ cudaError_t launch_vit_gemm(const CUtensorMap& a_hi, const CUtensorMap& a_lo, co
   }
   if (p.swap) GP_GEMM_PLANE_MODES(true, 256)
   if (p.f16) {
-    if (bn != 256) return cudaErrorInvalidValue;
     switch (p.mode) {
       GP_GEMM_CASE(false, 256, true, GEMM_PLANES_RELU)
       GP_GEMM_CASE(false, 256, true, GEMM_ROWS_F32_RELU)
@@ -495,7 +509,6 @@ cudaError_t launch_vit_gemm(const CUtensorMap& a_hi, const CUtensorMap& a_lo, co
     }
   }
   if (bn == 192) GP_GEMM_PLANE_MODES(false, 192)
-  if (bn == 128) GP_GEMM_PLANE_MODES(false, 128)
   switch (p.mode) {
     GP_GEMM_CASE(false, 256, false, GEMM_PLANES)
     GP_GEMM_CASE(false, 256, false, GEMM_PLANES_GELU)

@@ -369,8 +369,7 @@ class Engine:
         return ms.value
 
     def debug_sim_tiles(self) -> torch.Tensor:
-        """Raw fp32 similarity tiles [T, B(sorted by object), 256 t, 256 s] (tests only; B <= 32 = one query chunk)."""
-        assert self._B <= 32
+        """Raw fp32 similarity tiles [T, B(sorted by object), 256 t, 256 s] (tests only: 256 KiB per tile)."""
         tiles = self._empty((self.T, self._B, P, P), torch.float32)
         check(self.lib.gp_debug_sim_tiles(self._h, self._B, tiles.data_ptr(), self.stream))
         return tiles

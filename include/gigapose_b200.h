@@ -288,8 +288,41 @@ int gp_debug_gemm_timeline(long long* stamps64);
 int gp_debug_ist_trunk(gp_ist_trunk_handle_t h, int n, const float* crops, int num_convs, float* activation, void* stream);
 
 /* test hook: runs the similarity kernel and additionally dumps the raw fp32 similarity tiles, laid out
- * [item = n * B + j][256 t][256 s] where j indexes the queries sorted by object id (B <= 32, small sizes only). */
+ * [n * B + j][256 t][256 s] where j indexes the queries sorted by object id (small sizes only). */
 int gp_debug_sim_tiles(gp_handle_t h, int B, float* tiles, void* stream);
+
+/* test hook: one launch of the wgmma GEMM of the ViT / IST paths on caller-made operand planes,
+ * C[M,N] = A[M,K] . W[N,K]^T (+ the fused epilogue of `mode`).  Planes are bf16 (f16 = 0) or IEEE fp16 (f16 = 1)
+ * hi / lo pairs, dense row-major; every pointer is a device pointer.  Fields mirror the non-convolution part of the
+ * internal GEMM parameters:
+ *   mode       0 planes, 1 planes + erf-GELU, 2 x += gamma * (acc + bias), 3 patch embedding (row remap + pos table),
+ *              4 QKV head-major scatter, 5 planes + ReLU, 6 planes + residual planes + ReLU, 7 fp32 rows, 8 fp32 rows + ReLU
+ *   bn         output-tile width, 192 or 256 (0 = 256)
+ *   swap       1: A is the 128-row operand and the outputs are written transposed, as planes [N, M]; bias is per row of A
+ *   acc_scale  0 = off, else C = acc * acc_scale + bias
+ *   m_dev      nullable device int32: the rows computed are min(*m_dev, M)
+ * Unsupported combinations are rejected with GP_ERR_INVALID before any device is touched. */
+typedef struct gp_debug_gemm {
+  int32_t M, N, K, bn, passes, mode, swap, f16;
+  float acc_scale;
+  const uint16_t *a_hi, *a_lo;   /* [M,K] */
+  const uint16_t *w_hi, *w_lo;   /* [N,K] */
+  uint16_t *out_hi, *out_lo;     /* output planes (modes 0, 1, 4, 5, 6) */
+  const float* bias;             /* [N] ([M] when swap) */
+  const float* gamma;            /* [N] (mode 2) */
+  float* x;                      /* fp32 rows (modes 2, 3, 7, 8) */
+  const float* pos;              /* [tokens_per_img, N] (mode 3) */
+  const uint16_t *res_hi, *res_lo;   /* residual planes, same layout as the output planes (mode 6) */
+  const int32_t* m_dev;
+  int32_t tokens_per_img, patches_per_img, qkv_crop_stride;
+} gp_debug_gemm_t;
+int gp_debug_gemm(const gp_debug_gemm_t* g, void* stream);
+
+/* test hook: the multi-head attention kernel of the ViT alone.  qkv_hi / qkv_lo: bf16 planes in the head-major layout
+ * the QKV projection writes, [3 (q|k|v)][crop_stride][16 heads][257 tokens][64]; the first b crops are attended.
+ * out_hi / out_lo: bf16 planes [b * 257, 1024] (token rows, head h in columns [64 h, 64 h + 64)).  passes: 3 or 1. */
+int gp_debug_attention(int b, int crop_stride, int passes, const uint16_t* qkv_hi, const uint16_t* qkv_lo, uint16_t* out_hi,
+                       uint16_t* out_lo, void* stream);
 
 #ifdef __cplusplus
 }

@@ -11,12 +11,13 @@ FLOAT_KEYS = ["score_src", "score_pts", "relScale", "relInplane", "M", "scores",
 
 
 def engine_from_case(case: synth.FeatureCase, device="cuda:0", precision="fp32_split", regressor=None,
-                     shard_rank=0, shard_world=1, max_batch=None) -> Engine:
+                     shard_rank=0, shard_world=1, max_batch=None, **cfg) -> Engine:
     """Loads the (already unit-norm, patch-major) synthetic bank; the kernel applies the matching-time
-    normalisation (matching.py:229), i.e. norm_passes=1, exactly like the oracle does on the same tensors."""
+    normalisation (matching.py:229), i.e. norm_passes=1, exactly like the oracle does on the same tensors.
+    `cfg`: further Engine settings (sim_threshold, ...)."""
     local = list(range(shard_rank, case.T, shard_world))
     eng = Engine(case.O, len(local), max_batch or case.B, device=device, precision=precision,
-                 shard_rank=shard_rank, shard_world=shard_world, num_templates_global=case.T)
+                 shard_rank=shard_rank, shard_world=shard_world, num_templates_global=case.T, **cfg)
     sel = torch.tensor(local)
     for o in range(case.O):
         eng.bank_write(o, 0, case.bank_feat[o, sel], case.bank_mask16[o, sel].reshape(-1, 16, 16),

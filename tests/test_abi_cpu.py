@@ -91,3 +91,65 @@ def test_abi_v2_config_and_argument_checks_need_no_gpu(lib):
     assert lib.gp_allgather(None, None, None, 0, None) == -1
     assert lib.gp_normalize_patch_tokens(0, None, None, None) == -1
     assert lib.gp_bank_write_ist(None, 0, 0, 1, None, 0, None) == -1
+
+
+def test_nan_similarity_threshold_is_rejected(lib):
+    """Every value fails `sim < NaN`, so a NaN threshold would silently keep every similarity; zero and negative
+    thresholds are legal (the reference accepts any float)."""
+    for thr, rc in ((float("nan"), -1), (0.0, 0), (-0.05, 0)):
+        cfg = _lib.GpConfig(abi_version=_lib.GP_ABI_VERSION, device=0, num_objects=2, num_templates=9,
+                            num_templates_global=9, template_id_stride=1, template_id_offset=0, max_batch=4, top_k=5,
+                            sim_threshold=thr, patch_threshold=3, pixel_threshold=14, patch_size=14, precision=0)
+        bank, ws = C.c_size_t(), C.c_size_t()
+        assert lib.gp_query_sizes(C.byref(cfg), C.byref(bank), C.byref(ws)) == rc, thr
+        if rc:
+            assert b"sim_threshold" in lib.gp_last_error()
+            assert lib.gp_create(C.byref(cfg), None, None, None) == -1
+
+
+def test_debug_kernel_entries_reject_bad_arguments_without_a_gpu(lib):
+    """gp_debug_gemm / gp_debug_attention check their arguments before they touch a device: an unsupported GEMM
+    configuration fails with GP_ERR_INVALID and says why."""
+    fake = 1 << 20                                   # never dereferenced: every call below fails validation first
+
+    def gemm(**kw):
+        g = dict(M=256, N=512, K=64, bn=256, passes=3, mode=_lib.GEMM_ROWS_F32, swap=0, f16=0, acc_scale=0.0,
+                 a_hi=fake, a_lo=fake, w_hi=fake, w_lo=fake, bias=fake, x=fake, out_hi=fake, out_lo=fake)
+        g.update(kw)
+        rc = lib.gp_debug_gemm(C.byref(_lib.GpDebugGemm(**g)), None)
+        return rc, lib.gp_last_error()
+
+    assert lib.gp_debug_gemm(None, None) == -1
+    cases = [
+        (dict(bn=128), b"bn"),                                            # the 128-column tiles are not instantiated
+        (dict(bn=64), b"bn"),
+        (dict(N=384), b"multiple of bn"),                                 # N % bn
+        (dict(bn=192, N=576, mode=_lib.GEMM_ROWS_F32), b"192"),           # bn = 192 has the plane modes only
+        (dict(K=48), b"K"),                                               # K % 32
+        (dict(K=0), b"K"),
+        (dict(passes=2), b"passes"),
+        (dict(mode=9), b"mode"),
+        (dict(swap=1, mode=_lib.GEMM_PLANES_GELU), b"swap"),              # swap with GELU
+        (dict(swap=1, M=200, mode=_lib.GEMM_PLANES), b"swap"),            # swap needs whole 128-row tiles
+        (dict(swap=1, f16=1, mode=_lib.GEMM_PLANES_RELU), b"swap"),
+        (dict(f16=1, bn=192, N=576, mode=_lib.GEMM_PLANES_RELU), b"f16"),  # f16 with bn = 192
+        (dict(f16=1, mode=_lib.GEMM_PLANES), b"f16"),
+        (dict(M=0), b"M"),
+        (dict(a_lo=None), b"null"),
+        (dict(bias=None), b"null"),
+        (dict(x=None), b"null output"),
+        (dict(mode=_lib.GEMM_PLANES, out_lo=None), b"null output"),
+        (dict(mode=_lib.GEMM_SCALE_RESIDUAL, gamma=None), b"gamma"),
+        (dict(mode=_lib.GEMM_PLANES_ADD_RELU, res_hi=fake, res_lo=None), b"residual"),
+        (dict(mode=_lib.GEMM_QKV_HEADS, N=1024, tokens_per_img=257, qkv_crop_stride=1), b"3072"),
+        (dict(mode=_lib.GEMM_PATCH_EMBED, pos=fake, tokens_per_img=256, patches_per_img=256), b"patch"),
+    ]
+    for kw, word in cases:
+        rc, msg = gemm(**kw)
+        assert rc == -1 and word in msg, (kw, rc, msg)
+    att = lambda b, stride, passes, hi=fake, lo=fake, oh=fake, ol=fake: lib.gp_debug_attention(b, stride, passes, hi, lo, oh, ol, None)
+    assert att(0, 5, 3) == -1
+    assert att(6, 5, 3) == -1 and b"crop_stride" in lib.gp_last_error()
+    assert att(1, 5, 2) == -1 and b"passes" in lib.gp_last_error()
+    for null in ("hi", "lo", "oh", "ol"):
+        assert att(1, 5, 3, **{null: None}) == -1 and b"null" in lib.gp_last_error()

@@ -45,8 +45,9 @@ def _compare(out, ref, pose_tol=1e-3):
         if not torch.equal(a, b.to(a.dtype)):
             bad[k] = int((a != b.to(a.dtype)).sum())
     for k in FLOAT_KEYS:
-        # M: the regressor's hidden layers run on tensor cores (fp16 hi/lo pairs, ~2e-5 on sigma: accumulation in the
-        # tensor core truncates), everything else is fp32 SIMT
+        # M, relScale, relInplane: the regressor runs as fp32 SIMT kernels by default; the looser bar covers its
+        # tensor-core form (GIGAPOSE_MLP_SIMT=0: fp16 hi/lo pairs, ~2e-5 on sigma, the tensor core's accumulation
+        # truncates).  Everything else is fp32 SIMT
         tol = pose_tol if k == "pred_poses" else (5e-5 if k in ("M", "relScale", "relInplane") else 2e-5)
         scale = 1.0
         if k == "pred_poses":                       # translations are in mm (~400): relative 1e-3 on t, abs on R
