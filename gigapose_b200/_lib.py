@@ -17,6 +17,7 @@ LAYOUT_PATCH_MAJOR = 1
 LAYOUT_VIT_TOKENS = 2
 PRECISION_FP32_SPLIT = 0
 PRECISION_BF16 = 1
+MAX_NUM_TEMPLATES = 12032      # GP_MAX_NUM_TEMPLATES: largest num_templates per handle
 
 
 class GpConfig(C.Structure):

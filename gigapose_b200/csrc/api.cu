@@ -232,6 +232,10 @@ int validate(const gp_config_t* cfg) {
   if (cfg->abi_version != GP_ABI_VERSION) return fail(GP_ERR_INVALID, "ABI version mismatch: %d vs %d", cfg->abi_version, GP_ABI_VERSION);
   if (cfg->num_objects < 1 || cfg->num_templates < 1 || cfg->max_batch < 1)
     return fail(GP_ERR_INVALID, "num_objects, num_templates and max_batch must be >= 1");
+  if (cfg->num_templates > GP_MAX_NUM_TEMPLATES)
+    return fail(GP_ERR_INVALID, "num_templates = %d exceeds GP_MAX_NUM_TEMPLATES = %d (the top-k selection holds one "
+                "score per template in shared memory); shard the bank over more handles", cfg->num_templates,
+                GP_MAX_NUM_TEMPLATES);
   if (cfg->top_k < 1 || cfg->top_k > 32) return fail(GP_ERR_INVALID, "top_k must be in [1,32]");
   if (cfg->num_templates_global < cfg->num_templates) return fail(GP_ERR_INVALID, "num_templates_global < num_templates");
   if (cfg->num_templates_global < cfg->top_k) return fail(GP_ERR_INVALID, "fewer templates than top_k (torch.topk would raise)");

@@ -16,6 +16,7 @@
 // as hi*hi + hi*lo + lo*hi in fp32 (3 tensor-core passes, ~2^-17 relative operand error), so the thresholded /
 // arg-max'ed results agree with the reference's fp32 einsum up to fp32 accumulation-order noise.  `passes = 1`
 // runs hi*hi only (plain bf16 tensor-core similarity, 3x less tensor work, not index-exact).
+#include "../../include/gigapose_b200.h"
 #include "gigapose_kernels.h"
 #include "common.cuh"
 #include "wgmma.cuh"
@@ -432,6 +433,7 @@ cudaError_t launch_sim_search(const CUtensorMap& q_hi, const CUtensorMap& q_lo, 
 
 cudaError_t launch_topk_select(const TopkSelectParams& p, cudaStream_t stream) {
   if (p.B <= 0) return cudaSuccess;
+  if (p.T > GP_MAX_NUM_TEMPLATES) return cudaErrorInvalidValue;     // s_val[T] must fit the default 48 KiB
   topk_select_kernel<<<p.B, 256, p.T * sizeof(float), stream>>>(p);
   return cudaGetLastError();
 }

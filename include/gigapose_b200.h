@@ -30,6 +30,9 @@ extern "C" {
 #define GP_NUM_PATCHES 256   /* 16 x 16 patches of a 224 x 224 crop, patch size 14 */
 #define GP_AE_DIM 1024       /* DINOv2 ViT-L/14 descriptor size (configs/model/ae_net/dinov2_l.yaml:10) */
 #define GP_IST_DIM 256       /* IST descriptor size (configs/model/ist_net/resnet.yaml:3) */
+/* largest num_templates per handle: the top-k selection keeps one float per template in the 48 KiB of shared memory a
+ * kernel gets without opting in, minus 1 KiB left for its static shared memory: (48 - 1) KiB / 4 B */
+#define GP_MAX_NUM_TEMPLATES 12032
 
 typedef enum gp_status {
   GP_OK = 0,
@@ -55,7 +58,8 @@ typedef struct gp_config {
   int32_t abi_version;        /* GP_ABI_VERSION */
   int32_t device;             /* CUDA device ordinal */
   int32_t num_objects;        /* O */
-  int32_t num_templates;      /* templates per object held by THIS handle (T, or the shard size on multi-GPU) */
+  int32_t num_templates;      /* templates per object held by THIS handle (T, or the shard size on multi-GPU),
+                                 <= GP_MAX_NUM_TEMPLATES */
   int32_t num_templates_global; /* templates per object over all shards (== num_templates on one GPU) */
   int32_t template_id_stride; /* global template id = local id * stride + offset (template-interleaved shards) */
   int32_t template_id_offset;

@@ -107,6 +107,23 @@ def test_nan_similarity_threshold_is_rejected(lib):
             assert lib.gp_create(C.byref(cfg), None, None, None) == -1
 
 
+def test_num_templates_beyond_the_topk_shared_memory_is_rejected(lib):
+    """topk_select_kernel keeps one float per template in the default 48 KiB of shared memory: the largest accepted
+    num_templates is MAX_NUM_TEMPLATES (12 032 = 47 KiB / 4), and one more fails at configuration time, naming
+    num_templates, instead of at the first search."""
+    for T, rc in ((_lib.MAX_NUM_TEMPLATES, 0), (_lib.MAX_NUM_TEMPLATES + 1, -1)):
+        cfg = _lib.GpConfig(abi_version=_lib.GP_ABI_VERSION, device=0, num_objects=1, num_templates=T,
+                            num_templates_global=T, template_id_stride=1, template_id_offset=0, max_batch=1, top_k=5,
+                            sim_threshold=0.5, patch_threshold=3, pixel_threshold=14, patch_size=14, precision=0)
+        bank, ws = C.c_size_t(), C.c_size_t()
+        assert lib.gp_query_sizes(C.byref(cfg), C.byref(bank), C.byref(ws)) == rc, T
+        if rc:
+            assert b"num_templates" in lib.gp_last_error()
+            assert lib.gp_create(C.byref(cfg), None, None, None) == -1
+        else:
+            assert bank.value >= T * 256 * 1024 * 4          # the two bf16 descriptor planes
+
+
 def test_debug_kernel_entries_reject_bad_arguments_without_a_gpu(lib):
     """gp_debug_gemm / gp_debug_attention check their arguments before they touch a device: an unsupported GEMM
     configuration fails with GP_ERR_INVALID and says why."""
