@@ -105,7 +105,11 @@ SYMBOLS = {
     "gp_debug_gemm_timeline": (C.c_int, [C.c_void_p]),
     "gp_crop_resize_pad": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                      C.c_float, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
-    "gp_ist_trunk_query_sizes": (C.c_int, [C.c_int, C.POINTER(C.c_size_t), C.POINTER(C.c_size_t)]),
+    "gp_render_query_sizes": (C.c_int, [C.c_int, C.c_int, C.c_int, C.POINTER(C.c_size_t)]),
+    "gp_render_templates": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p,
+                                      C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
+                                      C.c_float, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "gp_ist_trunk_query_sizes":(C.c_int, [C.c_int, C.POINTER(C.c_size_t), C.POINTER(C.c_size_t)]),
     "gp_ist_trunk_create": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                       C.POINTER(C.c_void_p)]),
     "gp_ist_trunk_destroy": (C.c_int, [C.c_void_p]),

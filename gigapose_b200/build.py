@@ -8,7 +8,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libgigapose_b200.so")
-SOURCES = ["api.cu", "sim_search.cu", "prep.cu", "ist_mlp.cu", "ransac_pose.cu", "vit_gemm.cu", "vit_ops.cu", "vit_attention_tc.cu", "vit_api.cu", "ist_trunk.cu", "preprocess.cu"]
+SOURCES = ["api.cu", "sim_search.cu", "prep.cu", "ist_mlp.cu", "ransac_pose.cu", "vit_gemm.cu", "vit_ops.cu", "vit_attention_tc.cu", "vit_api.cu", "ist_trunk.cu", "preprocess.cu", "render.cu"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
               "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr"]
 

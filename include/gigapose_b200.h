@@ -272,6 +272,24 @@ int gp_crop_resize_pad(int n, int channels, int height, int width, int target_si
                        const float* post_sub, const float* post_div, float* out_images, float* out_mask, float* out_M,
                        void* stream);
 
+/* --- row f5: template renders from a CAD mesh (the Panda3D call of src/custom_megapose/call_panda3d.py:45-59 plus the
+ * PNG round trip and bounding box of custom_megapose/template_dataset.py:66-119).  The full contract is the header
+ * comment of gigapose_b200/csrc/render.cu.  Needs no handle. ------------------------------------------------------ */
+/* Workspace bytes for up to `max_views` views of height x width: the per-sample key buffer, 8 B x 4 samples x H x W
+ * per view. */
+int gp_render_query_sizes(int max_views, int height, int width, size_t* workspace_bytes);
+/* Renders n_views views of one triangle mesh: vertices f32 [V,3], faces i32 [F,3]; shading from vertex_color f32
+ * [V,3], or texture f32 [tex_h,tex_w,3] (row 0 on top) with face_uv f32 [F,3,2], or constant_color f32 [3] (NULL =
+ * white); at most one of vertex_color / texture.  poses f32 [n,4,4] object -> camera (same length unit as the
+ * vertices), K f32 [3,3], z_near > 0 in that unit.  Outputs: rgba f32 [n,4,H,W], depth f32 [n,H,W] (may be NULL),
+ * boxes i64 [n,4] xyxy with exclusive max ((0, 0, W, H) for an empty view).  `workspace` holds
+ * gp_render_query_sizes(n_views, ...) bytes; after the call it starts with the key buffer u64 [n,H,W,4]
+ * ((float bits of z) << 32 | face id, all ones = background) of this call. */
+int gp_render_templates(int n_views, int height, int width, int num_vertices, const float* vertices, int num_faces,
+                        const int32_t* faces, const float* vertex_color, const float* face_uv, const float* texture,
+                        int tex_h, int tex_w, const float* constant_color, const float* poses, const float* K,
+                        float z_near, void* workspace, float* rgba, float* depth, int64_t* boxes, void* stream);
+
 /* --- diagnostics ----------------------------------------------------------------------------------------- */
 /* number of kernels this library has launched since load (all handles); used for bench.py's `gpu_launches` */
 uint64_t gp_launch_count(void);

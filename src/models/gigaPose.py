@@ -209,11 +209,37 @@ class GigaPose(LightningModule):
         Crop + resize + pad (`CropResizePad`, utils/crop.py:16-61) and the CLIP normalisation of the RGB channels
         (template.py:71-73) run as one gather kernel per object (`gp_crop_resize_pad`); the crops then stream through the
         ViT / IST encoders in full 64-crop chunks across object boundaries into the bank."""
+        return self._onboard(dataset_name, len(rgba), rgba[0].shape[0],
+                             lambda o: (rgba[o].to(self.device, non_blocking=True).float(), boxes[o]), K, poses)
+
+    @torch.no_grad()
+    def onboard_meshes(self, dataset_name, meshes, poses, K=None):
+        """Row f5: onboarding straight from CAD meshes, with no renderer outside this library.  Each object's template
+        views are rendered on the GPU (`gigapose_b200.render.render_templates`, 640 x 480, the reference's Panda3D
+        template set-up of call_panda3d.py:45-59) and stream through the same crop -> encoders -> bank sequence as
+        `onboard_templates`; only one object's renders are resident at a time.
+
+        meshes  list of PLY paths or `read_ply` dicts (vertices in the unit of the pose translations, mm for BOP),
+        poses   [T,4,4] (the same views for every object) or [O,T,4,4] object -> camera,
+        K       [3,3] template intrinsics, default the reference's (`render.TEMPLATE_K`)."""
+        from gigapose_b200.render import TEMPLATE_K, read_ply, render_templates
+        K = TEMPLATE_K if K is None else K
+        n_obj = len(meshes)
+        poses = torch.as_tensor(poses, dtype=torch.float32)
+        poses = poses.expand(n_obj, *poses.shape[-3:]) if poses.dim() == 3 else poses
+
+        def produce(o):
+            mesh = read_ply(meshes[o]) if isinstance(meshes[o], (str, os.PathLike)) else meshes[o]
+            r = render_templates(mesh, poses[o].to(self.device), K, device=self.device)
+            return r["rgba"], r["boxes"]
+
+        return self._onboard(dataset_name, n_obj, poses.shape[1], produce, K, poses)
+
+    def _onboard(self, dataset_name, n_obj, T, produce, K, poses):
+        """The body of both onboarding entry points: `produce(o)` -> (rgba [T,4,H,W] f32 on the device, boxes [T,4])."""
         from gigapose_b200.engine import Engine
         from gigapose_b200.preprocess import CLIP_MEAN, CLIP_STD, crop_resize_pad
         device = self.device
-        n_obj = len(rgba)
-        T = rgba[0].shape[0]
         metric = self.testing_metric
         eng = Engine(n_obj, T, self.max_dets_per_call, device=device, k=metric.k, sim_threshold=metric.sim_threshold,
                      patch_threshold=metric.patch_threshold, precision=getattr(metric, "precision", "fp32_split"))
@@ -222,7 +248,8 @@ class GigaPose(LightningModule):
         builder = _BankBuilder(self, eng)
         Ms = []
         for o in range(n_obj):
-            crop = crop_resize_pad(torch.as_tensor(boxes[o]), rgba[o].to(device, non_blocking=True).float(), 224,
+            rgba, boxes = produce(o)
+            crop = crop_resize_pad(torch.as_tensor(boxes), rgba, 224,
                                    mean=CLIP_MEAN + (0.0,), std=CLIP_STD + (1.0,))      # alpha channel passes through
             builder.add(o, crop["images"][:, :3], crop["images"][:, 3])
             Ms.append(crop["M"])
