@@ -47,7 +47,7 @@ class GpDebugGemm(C.Structure):
                 ("out_hi", C.c_void_p), ("out_lo", C.c_void_p), ("bias", C.c_void_p), ("gamma", C.c_void_p),
                 ("x", C.c_void_p), ("pos", C.c_void_p), ("res_hi", C.c_void_p), ("res_lo", C.c_void_p),
                 ("m_dev", C.c_void_p), ("tokens_per_img", C.c_int32), ("patches_per_img", C.c_int32),
-                ("qkv_crop_stride", C.c_int32)]
+                ("qkv_crop_stride", C.c_int32), ("stamp", C.c_int32)]
 
 
 # gp_debug_gemm_t.mode

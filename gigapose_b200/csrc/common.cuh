@@ -138,4 +138,11 @@ __device__ __forceinline__ void named_barrier_sync(uint32_t id, uint32_t nthread
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
 
+// Warpgroup register reallocation (executed by all 128 threads of a warpgroup): a producer warpgroup that only issues
+// TMA gives registers back so that the MMA warpgroups can hold their accumulators and the epilogue without spilling.
+template <uint32_t kRegs>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(kRegs)); }
+template <uint32_t kRegs>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(kRegs)); }
+
 }  // namespace gp

@@ -211,6 +211,7 @@ struct GemmParams {
   float acc_scale;            // 0 = off; else C = acc * acc_scale + bias (exact power of two undoing a scaled W operand)
   int f16;                    // operand (and output) planes hold IEEE fp16 hi/lo pairs instead of bf16: 22 significant bits
                               // for O(1)-range data (the IST MLP), wgmma with fp16 A/B formats
+  int stamp;                  // diagnostics: CTA 0 records its cycle timeline (gp_debug_gemm_timeline); 0 in production
 };
 // whether vit_gemm_kernel has an instantiation for p's (swap, bn, f16, mode) and p's shape tiles; `why` (nullable)
 // receives the reason when it does not.  Host-only: needs no device.
@@ -227,6 +228,6 @@ cudaError_t launch_attention_tc(const CUtensorMap& hi128, const CUtensorMap& lo1
                                 const CUtensorMap& lo16, const uint16_t* qkv_hi, const uint16_t* qkv_lo, uint16_t* out_hi,
                                 uint16_t* out_lo, int b, int crop_stride, int passes, cudaStream_t s);
 cudaError_t read_attention_stamps(long long* host32);
-cudaError_t read_gemm_stamps(long long* host64);
+cudaError_t read_gemm_stamps(long long* host128);
 
 }  // namespace gp

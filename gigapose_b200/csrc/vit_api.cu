@@ -168,10 +168,10 @@ int gp_debug_attention_timeline(long long* stamps32) {
   return GP_OK;
 }
 
-int gp_debug_gemm_timeline(long long* stamps64) {
-  if (!stamps64) return gp_internal_fail(GP_ERR_INVALID, "null argument");
+int gp_debug_gemm_timeline(long long* stamps128) {
+  if (!stamps128) return gp_internal_fail(GP_ERR_INVALID, "null argument");
   GPV_CUDA(cudaDeviceSynchronize());
-  GPV_CUDA(gp::read_gemm_stamps(stamps64));
+  GPV_CUDA(gp::read_gemm_stamps(stamps128));
   return GP_OK;
 }
 
@@ -182,6 +182,7 @@ int gp_debug_gemm(const gp_debug_gemm_t* d, void* stream) {
   g.acc_scale = d->acc_scale; g.bias = d->bias; g.gamma = d->gamma; g.x = d->x; g.out_hi = d->out_hi; g.out_lo = d->out_lo;
   g.pos = d->pos; g.res_hi = d->res_hi; g.res_lo = d->res_lo; g.m_dev = d->m_dev;
   g.tokens_per_img = d->tokens_per_img; g.patches_per_img = d->patches_per_img; g.qkv_crop_stride = d->qkv_crop_stride;
+  g.stamp = d->stamp;
   if (g.M < 1) return gp_internal_fail(GP_ERR_INVALID, "M must be >= 1");
   const char* why = nullptr;
   if (!gp::gemm_config_supported(g, &why)) return gp_internal_fail(GP_ERR_INVALID, "unsupported GEMM: %s", why);

@@ -5,15 +5,17 @@
 // C[M,N] = A[M,K] . W[N,K]^T with both operands stored as bf16 hi/lo planes (x = hi + lo to ~2^-17) and accumulated
 // as hi*hi + hi*lo + lo*hi in fp32 register accumulators -- the same fp32-faithful split as the similarity kernel
 // (`passes = 1` = plain bf16).  Persistent CTAs, one 128 x bn output tile at a time:
-//   warp 0      TMA producer   (32-column k-blocks, SWIZZLE_64B; A rows = 2-D boxes, or 4-D boxes of an NHWC plane when
-//                              the GEMM is a convolution: one box per filter tap and 32-channel block, zero fill = padding)
-//   warps 4-11  two consumer warpgroups: wgmma m64 x bn x k16 on rows [0,64) / [64,128) of the tile, then the epilogue
-//               (the accumulator goes through shared memory so that a thread owns one row: fused bias / GELU / ReLU /
-//               LayerScale + residual / shortcut / positional table -> fp32 rows or bf16 hi/lo planes for the next
-//               layer; stores are transposed through shared memory into full 64-byte segments).
-// The staged accumulator reuses the operand ring, so the producer starts the next tile's loads once the epilogue has
-// read it.  Two instantiation families: <swap=0> activation rows x output features; <swap=1> filters as the 128-row
-// operand against 256 output pixels (the 128-channel convolutions).
+//   warps 0-3   producer warpgroup (setmaxnreg down to 40): lane 0 of warp 0 issues the TMA loads (32-column k-blocks,
+//               SWIZZLE_64B; A rows = 2-D boxes, or 4-D boxes of an NHWC plane when the GEMM is a convolution: one box
+//               per filter tap and 32-channel block, zero fill = padding)
+//   warps 4-11  two consumer warpgroups (setmaxnreg up to 232): wgmma m64 x bn x k16 on rows [0,64) / [64,128) of the
+//               tile, then the epilogue straight from the accumulator fragments (fused bias / GELU / ReLU / LayerScale +
+//               residual / shortcut / positional table -> fp32 rows or bf16 hi/lo planes for the next layer).  Each warp
+//               handles its own 16 rows in 32-column chunks through a private staging buffer, so that every global
+//               access is a run of whole 32-byte sectors; residual inputs of a chunk are loaded one chunk ahead.
+// The epilogue never touches the operand ring: the producer streams the next tile's k-blocks while it runs.
+// Two instantiation families: <swap=0> activation rows x output features; <swap=1> filters as the 128-row operand
+// against 256 output pixels (the 128-channel convolutions).
 #include "gigapose_kernels.h"
 #include "common.cuh"
 #include "wgmma.cuh"
@@ -33,16 +35,21 @@ constexpr int kWPlane = kBN * kRowBytes;          // 16 KB
 constexpr int kStageBytes = 2 * kAPlane + 2 * kWPlane;   // 48 KB
 constexpr int kEpiWarps = 8;
 constexpr int kThreads = 4 * 32 + kEpiWarps * 32;
-constexpr int kAccPitch = kBN + 4;                // fp32 words per staged accumulator row (+16 B: conflict-free float4 reads)
-static_assert(kBM * kAccPitch * 4 <= kStages * kStageBytes, "the staged accumulator lives in the operand ring");
+constexpr int kProducerRegs = 40, kConsumerRegs = 232;
+static_assert(128 * kProducerRegs + kEpiWarps * 32 * kConsumerRegs <= 65536, "register file");
+// Per-warp staging of one 32-column chunk of the warp's 16 rows.  Row pitches keep the fragment-layout accesses free
+// of bank conflicts: bf16 planes 144 B (hi 64 B | lo 64 B | pad), fp32 rows 160 B (128 B | pad); the swapped form
+// holds 32 pixel rows of 80 B (16 channels hi 32 B | lo 32 B | pad).
+constexpr int kStagePitchPlanes = 144, kStagePitchF32 = 160, kStagePitchSwap = 80;
+constexpr int kStageBufBytes = 16 * kStagePitchF32;
+static_assert(16 * kStagePitchPlanes <= kStageBufBytes && 32 * kStagePitchSwap <= kStageBufBytes, "staging buffer");
 
 struct __align__(8) GemmSmemTail {
-  float bias_s[2][kBN];                           // per-tile bias / LayerScale columns
+  float bias_s[2][kBN];                           // per-tile bias / LayerScale columns, indexed by tile parity
   float gamma_s[2][kBN];
-  uint8_t stage_buf[kEpiWarps][32 * 80];          // per-warp transposition buffer: 32 rows x (64 B + 16 B pad)
+  uint8_t stage_buf[kEpiWarps][kStageBufBytes];
   uint64_t full_bar[kStages];
   uint64_t empty_bar[kStages];
-  uint64_t ring_free_bar;                         // the epilogue has read the staged accumulator
 };
 constexpr int kSmemBytes = 1024 + kStages * kStageBytes + sizeof(GemmSmemTail);
 
@@ -83,10 +90,12 @@ __device__ __forceinline__ uint32_t pack_bf16(__nv_bfloat16 a, __nv_bfloat16 b) 
 
 }  // namespace
 
-// cycle stamps of CTA 0 for the QKV-shaped GEMM (diagnostics: gp_debug_gemm_timeline): [tile][0..3] =
-// MMA start, MMA done, epilogue start, epilogue end; [63] = kernel start
-__device__ long long g_gemm_stamp[64];
-#define GSTAMP(i) do { if (blockIdx.x == 0 && p.N == 3072 && (i) < 64) g_gemm_stamp[i] = clock64(); } while (0)
+// cycle stamps of CTA 0 of a launch with GemmParams::stamp set (diagnostics: gp_debug_gemm_timeline), for the CTA's
+// first kStampTiles tiles: [4 * tile + {0: MMA start, 1: MMA done, 2: epilogue start, 3: epilogue end}],
+// [63] = kernel start, [64 + tile] = the tile's first k-block has landed (first full barrier passed)
+constexpr int kStampTiles = 15;
+__device__ long long g_gemm_stamp[128];
+#define GSTAMP(i) do { if (blockIdx.x == 0 && p.stamp) g_gemm_stamp[i] = clock64(); } while (0)
 
 // One k-block (32 columns of K, up to 3 split passes) of a consumer warpgroup's 64 x kN accumulator.
 template <int kN, bool kF16>
@@ -124,7 +133,6 @@ vit_gemm_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_consta
   pdl_trigger();                                     // the next kernel's CTAs may take SMs as this grid's CTAs retire
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   GemmSmemTail& tail = *reinterpret_cast<GemmSmemTail*>(smem + kStages * kStageBytes);
-  float* acc_s = reinterpret_cast<float*>(smem);     // [kBM][kAccPitch] staged accumulator (over the operand ring)
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int passes = p.passes;
   constexpr int bn = kTileN;
@@ -135,7 +143,6 @@ vit_gemm_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_consta
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < kStages; ++s) { mbar_init(&tail.full_bar[s], 1); mbar_init(&tail.empty_bar[s], kEpiWarps); }
-    mbar_init(&tail.ring_free_bar, kEpiWarps);
     fence_barrier_init();
   }
   if (warp == 0 && lane == 0) {
@@ -146,17 +153,17 @@ vit_gemm_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_consta
   pdl_wait();                                        // everything above overlapped the previous kernel's tail
   if (threadIdx.x == 0) GSTAMP(63);
 
-  if (warp == 0) {
-    if (lane == 0) {
-      int stage = 0; uint32_t phase = 0, unit = 0;
+  if (warp < 4) {
+    setmaxnreg_dec<kProducerRegs>();
+    if (warp == 0 && lane == 0) {
+      int stage = 0; uint32_t phase = 0;
       const uint32_t tx = (passes == 3 ? 2 : 1) * (kAPlane + bn * kRowBytes);
-      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++unit) {
+      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
         int mt, nt;
         tile_coords(tile, num_m, num_n, mt, nt);
         const int m0 = mt * kBM, n0 = nt * bn;
         int img = 0, y0 = 0;
         if (p.conv) { const int hw = p.Ho * p.Wo, pix0 = kSwap ? n0 : m0; img = pix0 / hw; y0 = (pix0 - img * hw) / p.Wo; }
-        if (unit > 0) mbar_wait(&tail.ring_free_bar, (unit - 1) & 1u);   // the previous tile's staged accumulator was read
         for (int kb = 0; kb < num_kb; ++kb) {
           mbar_wait(&tail.empty_bar[stage], phase ^ 1);
           uint8_t* st = smem + stage * kStageBytes;
@@ -192,22 +199,112 @@ vit_gemm_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_consta
         }
       }
     }
-  } else if (warp >= 4) {
-    const int e = warp - 4, q = e & 3, ch = e >> 2;
-    const int r = q * 32 + lane;                       // epilogue: this thread's row of the tile
-    const int etid = e * 32 + lane;
-    const int wg = e >> 2, wl = e & 3;                 // MMA: warpgroup wg owns tile rows [64 wg, 64 wg + 64)
+  } else {
+    setmaxnreg_inc<kConsumerRegs>();
+    const int e = warp - 4, etid = e * 32 + lane;
+    const int wg = e >> 2, wl = e & 3;                 // warpgroup wg owns tile rows [64 wg, 64 wg + 64)
+    const int wrow0 = wg * 64 + wl * 16;               // this warp's 16 rows of the tile (MMA fragments and epilogue)
+    const int fr = lane >> 2, fc = 2 * (lane & 3);     // fragment: rows wrow0 + fr (+ 8), columns 8 j + fc (+ 1)
+    constexpr bool kPlanesOut = kMode == GEMM_PLANES || kMode == GEMM_PLANES_GELU || kMode == GEMM_QKV_HEADS ||
+                                kMode == GEMM_PLANES_RELU || kMode == GEMM_PLANES_ADD_RELU;
+    constexpr bool kResIn = kMode == GEMM_SCALE_RESIDUAL || kMode == GEMM_PLANES_ADD_RELU;
+    constexpr int kChunks = kTileN / 32;
+    uint8_t* stg = tail.stage_buf[e];
     int stage = 0; uint32_t phase = 0, unit = 0;
     for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++unit) {
       const uint32_t acc_i = unit & 1u;
+      const bool stamp = e == 0 && lane == 0 && unit < kStampTiles;
       int mt, nt;
       tile_coords(tile, num_m, num_n, mt, nt);
-      if (e == 0 && lane == 0) GSTAMP(unit * 4 + 0);
+      const int m0 = mt * kBM, ntile0 = nt * bn;
+      if (stamp) GSTAMP(unit * 4 + 0);
+      // per-column vectors (or, swapped, the bias of the fragment's two channel rows): loaded now, used after the MMAs
+      float bias_v = 0.f, gamma_v = 0.f, bias_r[2] = {0.f, 0.f};
+      if (!kSwap && etid < bn) {
+        bias_v = __ldg(p.bias + ntile0 + etid);
+        if (kMode == GEMM_SCALE_RESIDUAL) gamma_v = __ldg(p.gamma + ntile0 + etid);
+      }
+      if (kSwap) { bias_r[0] = __ldg(p.bias + m0 + wrow0 + fr); bias_r[1] = __ldg(p.bias + m0 + wrow0 + fr + 8); }
+
+      // The four 16-byte pieces this lane moves between the staging buffer and global memory in every chunk.
+      // Row-major forms: piece k is in row 4 k + lane / 8 of the warp's 16; bf16 planes: lanes 0-3 / 4-7 of a row take
+      // the hi / lo plane, 64 B each; fp32: 8 lanes x 16 B = 128 B.  Swapped form: pixel 8 k + lane / 4 of the chunk's
+      // 32, lanes 0-1 / 2-3 take the 32 bytes (16 channels) of the hi / lo plane.
+      size_t row_off[4];                               // element offset of the piece's output row (row-major forms)
+      uint32_t row_ok = 0;
+#pragma unroll
+      for (int k = 0; k < 4; ++k) {
+        row_off[k] = 0;
+        if constexpr (!kSwap) {
+          const int m = m0 + wrow0 + 4 * k + (lane >> 3);
+          if (m < M_rows) row_ok |= 1u << k;
+          if (kMode == GEMM_QKV_HEADS) {               // head-major: [q|k|v][crop][head][token][64]
+            const int img = m / p.tokens_per_img, tok = m - img * p.tokens_per_img;
+            row_off[k] = ((size_t)img * 16 * p.tokens_per_img + tok) * 64;
+          } else if (kMode == GEMM_PATCH_EMBED) {      // patch row -> token row (CLS first)
+            const int img = m / p.patches_per_img, pp = m - img * p.patches_per_img;
+            row_off[k] = ((size_t)img * p.tokens_per_img + 1 + pp) * p.N;
+          } else {
+            row_off[k] = (size_t)m * p.N;
+          }
+        } else {
+          row_ok |= 1u << k;                           // swap: M % 128 == 0 and N % 256 == 0, no partial tiles
+        }
+      }
+      auto piece_smem = [&](int k) -> uint8_t* {
+        if constexpr (kSwap) return stg + (8 * k + (lane >> 2)) * kStagePitchSwap + (lane & 3) * 16;
+        else if constexpr (kPlanesOut) return stg + (4 * k + (lane >> 3)) * kStagePitchPlanes + (lane & 7) * 16;
+        else return stg + (4 * k + (lane >> 3)) * kStagePitchF32 + (lane & 7) * 16;
+      };
+      // byte address of piece k of chunk c in the fp32 rows `x` or in the plane pair (hi, lo)
+      auto piece_gmem = [&](int k, int c, const void* x, const void* hi, const void* lo) -> const uint8_t* {
+        if constexpr (kSwap) {
+          const size_t pix = (size_t)ntile0 + c * 32 + 8 * k + (lane >> 2);
+          const void* plane = (lane & 2) ? lo : hi;
+          return reinterpret_cast<const uint8_t*>(plane) + (pix * p.M + m0 + wrow0) * 2 + (lane & 1) * 16;
+        } else {
+          const int n = ntile0 + c * 32;
+          size_t col = (size_t)n;
+          if (kMode == GEMM_QKV_HEADS) {
+            const int which = n >> 10, head = (n & 1023) >> 6;
+            col = ((size_t)which * p.qkv_crop_stride * 16 + head) * p.tokens_per_img * 64 + (n & 63);
+          }
+          if constexpr (kPlanesOut) {
+            const void* plane = (lane & 4) ? lo : hi;
+            return reinterpret_cast<const uint8_t*>(plane) + (row_off[k] + col) * 2 + (lane & 3) * 16;
+          } else {
+            return reinterpret_cast<const uint8_t*>(x) + (row_off[k] + col) * 4 + (lane & 7) * 16;
+          }
+        }
+      };
+      // residual inputs (x += ... / the shortcut planes) of a chunk, one chunk ahead of its use
+      uint4 res[4];
+      auto load_res = [&](int c) {
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+          res[k] = make_uint4(0, 0, 0, 0);
+          if ((row_ok >> k) & 1u) res[k] = *reinterpret_cast<const uint4*>(piece_gmem(k, c, p.x, p.res_hi, p.res_lo));
+        }
+      };
+      // patch embedding: the positional-table rows of the fragment's two rows
+      const float* pos_row[2] = {nullptr, nullptr};
+      bool frag_row_ok[2] = {false, false};
+      if (kMode == GEMM_PATCH_EMBED) {
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int m = m0 + wrow0 + fr + 8 * h;
+          const int img = m / p.patches_per_img, pp = m - img * p.patches_per_img;
+          pos_row[h] = p.pos + (size_t)(1 + pp) * p.N;
+          frag_row_ok[h] = m < M_rows;
+        }
+      }
+
       // ---------------- main loop: wgmma from the operand ring into registers
       float frag[kTileN / 2];
       int prev_stage = -1;
       for (int kb = 0; kb < num_kb; ++kb) {
         mbar_wait(&tail.full_bar[stage], phase);
+        if (kb == 0 && stamp) GSTAMP(64 + unit);
         const uint32_t st = smem_u32(smem + stage * kStageBytes);
         const uint32_t a_hi = st + wg * (kAPlane / 2), a_lo = a_hi + kAPlane;
         const uint32_t w_hi = st + 2 * kAPlane, w_lo = w_hi + kWPlane;
@@ -220,230 +317,113 @@ vit_gemm_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_consta
         prev_stage = stage;
         if (++stage == kStages) { stage = 0; phase ^= 1; }
       }
+      if (kResIn) load_res(0);                         // in flight while the last k-block's MMAs retire
       wgmma_wait<0>();
       acc_fence(frag);
       if (lane == 0) mbar_arrive(&tail.empty_bar[prev_stage]);
-      if (e == 0 && lane == 0) GSTAMP(unit * 4 + 1);
-      // ---------------- stage the accumulator (row-major fp32) and the per-column vectors
-      named_barrier_sync(1, kEpiWarps * 32);           // both warpgroups are done reading the ring
-      {
-        const int row0 = wg * 64 + wl * 16 + (lane >> 2), col0 = 2 * (lane & 3);
-#pragma unroll
-        for (int j8 = 0; j8 < kTileN / 8; ++j8) {
-          {
-            *reinterpret_cast<float2*>(acc_s + row0 * kAccPitch + j8 * 8 + col0) = make_float2(frag[4 * j8], frag[4 * j8 + 1]);
-            *reinterpret_cast<float2*>(acc_s + (row0 + 8) * kAccPitch + j8 * 8 + col0) = make_float2(frag[4 * j8 + 2], frag[4 * j8 + 3]);
-          }
-        }
-      }
-      const int ntile0 = nt * bn;
+      if (stamp) GSTAMP(unit * 4 + 1);
       if (!kSwap && etid < bn) {
-        tail.bias_s[acc_i][etid] = __ldg(p.bias + ntile0 + etid);
-        if (kMode == GEMM_SCALE_RESIDUAL) tail.gamma_s[acc_i][etid] = __ldg(p.gamma + ntile0 + etid);
+        tail.bias_s[acc_i][etid] = bias_v;
+        if (kMode == GEMM_SCALE_RESIDUAL) tail.gamma_s[acc_i][etid] = gamma_v;
       }
+      // the vectors are visible to both warpgroups; since every warp has passed this barrier, none still reads the
+      // other parity's vectors of the tile before
       named_barrier_sync(1, kEpiWarps * 32);
-      if (e == 0 && lane == 0) GSTAMP(unit * 4 + 2);
-      // ---------------- epilogue: thread = row r, columns [ch * bn/2, (ch + 1) * bn/2) in chunks of 32
-      const uint32_t acc = acc_i;
-      const int m = mt * kBM + r;
-      const int half_cols = bn >> 1;                   // columns per epilogue warp: 96 / 128
-      const int n0 = ntile0 + ch * half_cols;
-      const float* sb = tail.bias_s[acc] + ch * half_cols;
-      const float* sg = tail.gamma_s[acc] + ch * half_cols;
-      const bool row_ok = m < M_rows;
-      size_t out_row = (size_t)m;
-      const float* pos_row = nullptr;
-      if (kMode == GEMM_PATCH_EMBED) {                // patch row -> token row (CLS first), + positional table
-        const int img = m / p.patches_per_img, pp = m - img * p.patches_per_img;
-        out_row = (size_t)img * p.tokens_per_img + 1 + pp;
-        pos_row = p.pos + (size_t)(1 + pp) * p.N;
-      }
+      if (stamp) GSTAMP(unit * 4 + 2);
 
-      uint8_t* stg = tail.stage_buf[e];
-      const unsigned okmask = __ballot_sync(0xffffffffu, row_ok);
-      // One warp-wide store instruction of the natural "thread = row" mapping touches 32 different rows with 16 bytes
-      // each (32 half-written sectors).  Rows are therefore transposed through a small smem buffer so that 4 (bf16
-      // planes) or 4 (fp32, in two 16-column halves) consecutive lanes cover one contiguous 64-byte row segment:
-      // every global transaction is a fully written 32-byte sector and an instruction touches 8 rows instead of 32.
-      auto store_rows_64B = [&](const uint32_t (&w)[16], uint8_t* base, size_t row_byte_off) {
-        uint4* srow = reinterpret_cast<uint4*>(stg + lane * 80);
+      // ---------------- epilogue, 32 columns at a time: residual in -> fragment math -> staging -> global
+      const float* sb = tail.bias_s[acc_i];
+      const float* sg = tail.gamma_s[acc_i];
 #pragma unroll
-        for (int j = 0; j < 4; ++j) srow[j] = make_uint4(w[4 * j], w[4 * j + 1], w[4 * j + 2], w[4 * j + 3]);
-        __syncwarp();
-        const uint32_t off_lo = (uint32_t)row_byte_off, off_hi = (uint32_t)(row_byte_off >> 32);
+      for (int c = 0; c < kChunks; ++c) {
+        if (kResIn) {
 #pragma unroll
-        for (int it = 0; it < 4; ++it) {
-          const int rr = it * 8 + (lane >> 2), piece = lane & 3;
-          const uint4 val = *reinterpret_cast<const uint4*>(stg + rr * 80 + piece * 16);
-          const size_t o = ((size_t)__shfl_sync(0xffffffffu, off_hi, rr) << 32) | __shfl_sync(0xffffffffu, off_lo, rr);
-          if ((okmask >> rr) & 1u) *reinterpret_cast<uint4*>(base + o + piece * 16) = val;
+          for (int k = 0; k < 4; ++k) *reinterpret_cast<uint4*>(piece_smem(k)) = res[k];
+          if (c + 1 < kChunks) load_res(c + 1);
+          __syncwarp();
         }
-        __syncwarp();
-      };
-      auto load_rows_64B = [&](uint32_t (&w)[16], const uint8_t* base, size_t row_byte_off) {
-        const uint32_t off_lo = (uint32_t)row_byte_off, off_hi = (uint32_t)(row_byte_off >> 32);
 #pragma unroll
-        for (int it = 0; it < 4; ++it) {
-          const int rr = it * 8 + (lane >> 2), piece = lane & 3;
-          const size_t o = ((size_t)__shfl_sync(0xffffffffu, off_hi, rr) << 32) | __shfl_sync(0xffffffffu, off_lo, rr);
-          uint4 val = make_uint4(0, 0, 0, 0);
-          if ((okmask >> rr) & 1u) val = *reinterpret_cast<const uint4*>(base + o + piece * 16);
-          *reinterpret_cast<uint4*>(stg + rr * 80 + piece * 16) = val;
-        }
-        __syncwarp();
-        const uint4* srow = reinterpret_cast<const uint4*>(stg + lane * 80);
+        for (int jj = 0; jj < 4; ++jj) {
+          const int j8 = c * 4 + jj;
 #pragma unroll
-        for (int j = 0; j < 4; ++j) { const uint4 t = srow[j]; w[4 * j] = t.x; w[4 * j + 1] = t.y; w[4 * j + 2] = t.z; w[4 * j + 3] = t.w; }
-        __syncwarp();
-      };
-
-      // kSwap: thread = output channel m, the 32 columns of a chunk are 32 consecutive output pixels; every value is
-      // transposed through the warp's smem buffer so that a pixel's 32 channels leave as one 64-byte NHWC segment
-      auto process_swapped = [&](uint32_t (&v32)[32], int c0) {
-        const size_t pix = (size_t)(n0 + c0);
-        const size_t cbase = (size_t)(mt * kBM + q * 32);
-        const float bias_r = __ldg(p.bias + m);
-        float v[32];
+          for (int h = 0; h < 2; ++h) {
+            const float a0 = frag[4 * j8 + 2 * h], a1 = frag[4 * j8 + 2 * h + 1];
+            const int rr = fr + 8 * h;                 // row of the warp's 16
+            if constexpr (kSwap) {
+              // thread = output channels rr, columns = pixels: the values land in their NHWC pixel rows
+              float v[2] = {a0 + bias_r[h], a1 + bias_r[h]};
 #pragma unroll
-        for (int j = 0; j < 32; ++j) v[j] = __uint_as_float(v32[j]) + bias_r;
-        auto rows_in = [&](const uint16_t* plane) {          // v[j] += plane[pix + j][channel of this lane]
-#pragma unroll
-          for (int it = 0; it < 4; ++it) {
-            const int rr = it * 8 + (lane >> 2), piece = lane & 3;
-            *reinterpret_cast<uint4*>(stg + rr * 80 + piece * 16) =
-                *reinterpret_cast<const uint4*>(reinterpret_cast<const uint8_t*>(plane) + ((pix + rr) * p.M + cbase) * 2 + piece * 16);
-          }
-          __syncwarp();
-#pragma unroll
-          for (int j = 0; j < 32; ++j)
-            v[j] += __uint_as_float((uint32_t)*reinterpret_cast<const uint16_t*>(stg + j * 80 + lane * 2) << 16);
-          __syncwarp();
-        };
-        if (kMode == GEMM_PLANES_ADD_RELU) { rows_in(p.res_hi); rows_in(p.res_lo); }
-        if (kMode == GEMM_PLANES_RELU || kMode == GEMM_PLANES_ADD_RELU) {
-#pragma unroll
-          for (int j = 0; j < 32; ++j) v[j] = fmaxf(v[j], 0.f);
-        }
-        auto rows_out = [&](uint16_t* plane, bool low) {
-#pragma unroll
-          for (int j = 0; j < 32; ++j) {
-            const __nv_bfloat16 h = __float2bfloat16_rn(v[j]);
-            const __nv_bfloat16 o = low ? __float2bfloat16_rn(v[j] - __bfloat162float(h)) : h;
-            *reinterpret_cast<uint16_t*>(stg + j * 80 + lane * 2) = __bfloat16_as_ushort(o);
-          }
-          __syncwarp();
-#pragma unroll
-          for (int it = 0; it < 4; ++it) {
-            const int rr = it * 8 + (lane >> 2), piece = lane & 3;
-            *reinterpret_cast<uint4*>(reinterpret_cast<uint8_t*>(plane) + ((pix + rr) * p.M + cbase) * 2 + piece * 16) =
-                *reinterpret_cast<const uint4*>(stg + rr * 80 + piece * 16);
-          }
-          __syncwarp();
-        };
-        rows_out(p.out_hi, false);
-        rows_out(p.out_lo, true);
-      };
-
-      auto process = [&](uint32_t (&v32)[32], int c0) {
-        if constexpr (kSwap) { process_swapped(v32, c0); return; }
-        const int n = n0 + c0;
-        float v[32];
-#pragma unroll
-        for (int j = 0; j < 32; ++j)
-          v[j] = (p.acc_scale != 0.f ? __uint_as_float(v32[j]) * p.acc_scale : __uint_as_float(v32[j])) + sb[c0 + j];
-        if (kMode == GEMM_PLANES || kMode == GEMM_PLANES_GELU || kMode == GEMM_QKV_HEADS || kMode == GEMM_PLANES_RELU ||
-            kMode == GEMM_PLANES_ADD_RELU) {
-          uint32_t hi[16], lo[16];
-          if (kMode == GEMM_PLANES_ADD_RELU) {          // BasicBlock: relu(shortcut + bn2(conv2(.)))   (resnet.py:45-50)
-            const size_t rb = (out_row * p.N + n) * 2;
-            load_rows_64B(hi, reinterpret_cast<const uint8_t*>(p.res_hi), rb);
-            load_rows_64B(lo, reinterpret_cast<const uint8_t*>(p.res_lo), rb);
-#pragma unroll
-            for (int j = 0; j < 16; ++j) {
-              v[2 * j] += __uint_as_float(hi[j] << 16) + __uint_as_float(lo[j] << 16);
-              v[2 * j + 1] += __uint_as_float(hi[j] & 0xffff0000u) + __uint_as_float(lo[j] & 0xffff0000u);
-            }
-          }
-#pragma unroll
-          for (int j = 0; j < 32; j += 2) {
-            float a = v[j], b = v[j + 1];
-            if (kMode == GEMM_PLANES_GELU) { a = gelu_erf(a); b = gelu_erf(b); }
-            if (kMode == GEMM_PLANES_RELU || kMode == GEMM_PLANES_ADD_RELU) { a = fmaxf(a, 0.f); b = fmaxf(b, 0.f); }
-            if constexpr (kF16) {                    // saturating: a value beyond the fp16 range stays finite (and wrong) instead of inf
-              a = fminf(fmaxf(a, -65504.f), 65504.f);
-              b = fminf(fmaxf(b, -65504.f), 65504.f);
-              const __half ah = __float2half_rn(a), bh = __float2half_rn(b);
-              hi[j >> 1] = (uint32_t)__half_as_ushort(ah) | ((uint32_t)__half_as_ushort(bh) << 16);
-              lo[j >> 1] = (uint32_t)__half_as_ushort(__float2half_rn(a - __half2float(ah))) |
-                           ((uint32_t)__half_as_ushort(__float2half_rn(b - __half2float(bh))) << 16);
+              for (int i = 0; i < 2; ++i) {
+                uint8_t* px = stg + (jj * 8 + fc + i) * kStagePitchSwap + rr * 2;
+                if (kMode == GEMM_PLANES_ADD_RELU) {
+                  v[i] += __uint_as_float((uint32_t)*reinterpret_cast<const uint16_t*>(px) << 16);
+                  v[i] += __uint_as_float((uint32_t)*reinterpret_cast<const uint16_t*>(px + 32) << 16);
+                }
+                if (kMode == GEMM_PLANES_RELU || kMode == GEMM_PLANES_ADD_RELU) v[i] = fmaxf(v[i], 0.f);
+                const __nv_bfloat16 hb = __float2bfloat16_rn(v[i]);
+                *reinterpret_cast<uint16_t*>(px) = __bfloat16_as_ushort(hb);
+                *reinterpret_cast<uint16_t*>(px + 32) = __bfloat16_as_ushort(__float2bfloat16_rn(v[i] - __bfloat162float(hb)));
+              }
             } else {
-              const __nv_bfloat16 ah = __float2bfloat16_rn(a), bh = __float2bfloat16_rn(b);
-              hi[j >> 1] = pack_bf16(ah, bh);
-              lo[j >> 1] = pack_bf16(__float2bfloat16_rn(a - __bfloat162float(ah)), __float2bfloat16_rn(b - __bfloat162float(bh)));
+              const int col = c * 32 + jj * 8 + fc;    // column of the tile
+              const float2 bb = *reinterpret_cast<const float2*>(sb + col);
+              float v0 = (p.acc_scale != 0.f ? a0 * p.acc_scale : a0) + bb.x;
+              float v1 = (p.acc_scale != 0.f ? a1 * p.acc_scale : a1) + bb.y;
+              if constexpr (kPlanesOut) {
+                uint32_t* w_hi = reinterpret_cast<uint32_t*>(stg + rr * kStagePitchPlanes + (jj * 8 + fc) * 2);
+                uint32_t* w_lo = w_hi + 16;
+                if (kMode == GEMM_PLANES_ADD_RELU) {   // BasicBlock: relu(shortcut + bn2(conv2(.)))   (resnet.py:45-50)
+                  const uint32_t rh = *w_hi, rl = *w_lo;
+                  v0 += __uint_as_float(rh << 16) + __uint_as_float(rl << 16);
+                  v1 += __uint_as_float(rh & 0xffff0000u) + __uint_as_float(rl & 0xffff0000u);
+                }
+                if (kMode == GEMM_PLANES_GELU) { v0 = gelu_erf(v0); v1 = gelu_erf(v1); }
+                if (kMode == GEMM_PLANES_RELU || kMode == GEMM_PLANES_ADD_RELU) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
+                if constexpr (kF16) {                  // saturating: a value beyond the fp16 range stays finite (and wrong) instead of inf
+                  v0 = fminf(fmaxf(v0, -65504.f), 65504.f);
+                  v1 = fminf(fmaxf(v1, -65504.f), 65504.f);
+                  const __half ah = __float2half_rn(v0), bh = __float2half_rn(v1);
+                  *w_hi = (uint32_t)__half_as_ushort(ah) | ((uint32_t)__half_as_ushort(bh) << 16);
+                  *w_lo = (uint32_t)__half_as_ushort(__float2half_rn(v0 - __half2float(ah))) |
+                          ((uint32_t)__half_as_ushort(__float2half_rn(v1 - __half2float(bh))) << 16);
+                } else {
+                  const __nv_bfloat16 ah = __float2bfloat16_rn(v0), bh = __float2bfloat16_rn(v1);
+                  *w_hi = pack_bf16(ah, bh);
+                  *w_lo = pack_bf16(__float2bfloat16_rn(v0 - __bfloat162float(ah)), __float2bfloat16_rn(v1 - __bfloat162float(bh)));
+                }
+              } else {
+                float2* w = reinterpret_cast<float2*>(stg + rr * kStagePitchF32 + (jj * 8 + fc) * 4);
+                float2 o;
+                if (kMode == GEMM_SCALE_RESIDUAL) {    // x += gamma * (acc + bias)   (blocks: ls1 / ls2 + residual)
+                  const float2 g = *reinterpret_cast<const float2*>(sg + col), xv = *w;
+                  o = make_float2(xv.x + g.x * v0, xv.y + g.y * v1);
+                } else if (kMode == GEMM_ROWS_F32 || kMode == GEMM_ROWS_F32_RELU) {   // plain fp32 rows (last 1x1
+                  const float floor_v = kMode == GEMM_ROWS_F32_RELU ? 0.f : -INFINITY;  // convolution of the IST trunk;
+                  o = make_float2(fmaxf(v0, floor_v), fmaxf(v1, floor_v));            // second hidden layer of the IST MLP)
+                } else {                               // GEMM_PATCH_EMBED: + positional table
+                  const int n = ntile0 + col;
+                  o = make_float2(v0 + (frag_row_ok[h] ? __ldg(pos_row[h] + n) : 0.f),
+                                  v1 + (frag_row_ok[h] ? __ldg(pos_row[h] + n + 1) : 0.f));
+                }
+                *w = o;
+              }
             }
           }
-          size_t dst = out_row * p.N + n;
-          if (kMode == GEMM_QKV_HEADS) {   // head-major: [q|k|v][crop][head][token][64] so that attention tiles are contiguous
-            const int which = n >> 10, head = (n & 1023) >> 6, d0 = n & 63;
-            const int img = m / p.tokens_per_img, tok = m - img * p.tokens_per_img;
-            dst = ((((size_t)which * p.qkv_crop_stride + img) * 16 + head) * p.tokens_per_img + tok) * 64 + d0;
-          }
-          store_rows_64B(hi, reinterpret_cast<uint8_t*>(p.out_hi), dst * 2);
-          store_rows_64B(lo, reinterpret_cast<uint8_t*>(p.out_lo), dst * 2);
-        } else if (kMode == GEMM_SCALE_RESIDUAL) {      // x += gamma * (acc + bias)   (blocks: ls1 / ls2 + residual)
-          const size_t rowb = (out_row * p.N + n) * 4;
-#pragma unroll
-          for (int half = 0; half < 2; ++half) {
-            uint32_t w[16];
-            load_rows_64B(w, reinterpret_cast<const uint8_t*>(p.x), rowb + half * 64);
-#pragma unroll
-            for (int j = 0; j < 16; ++j)
-              w[j] = __float_as_uint(__uint_as_float(w[j]) + sg[c0 + half * 16 + j] * v[half * 16 + j]);
-            store_rows_64B(w, reinterpret_cast<uint8_t*>(p.x), rowb + half * 64);
-          }
-        } else if (kMode == GEMM_ROWS_F32 || kMode == GEMM_ROWS_F32_RELU) {   // plain fp32 rows (last 1x1 convolution of the IST
-          const size_t rowb = (out_row * p.N + n) * 4;                          // trunk; second hidden layer of the IST MLP)
-          const float floor_v = kMode == GEMM_ROWS_F32_RELU ? 0.f : -INFINITY;
-#pragma unroll
-          for (int half = 0; half < 2; ++half) {
-            uint32_t w[16];
-#pragma unroll
-            for (int j = 0; j < 16; ++j) w[j] = __float_as_uint(fmaxf(v[half * 16 + j], floor_v));
-            store_rows_64B(w, reinterpret_cast<uint8_t*>(p.x), rowb + half * 64);
-          }
-        } else {                                          // GEMM_PATCH_EMBED
-          const size_t rowb = (out_row * p.N + n) * 4;
-#pragma unroll
-          for (int half = 0; half < 2; ++half) {
-            uint32_t w[16];
-#pragma unroll
-            for (int j = 0; j < 16; ++j)
-              w[j] = __float_as_uint(v[half * 16 + j] + (row_ok ? __ldg(pos_row + n + half * 16 + j) : 0.f));
-            store_rows_64B(w, reinterpret_cast<uint8_t*>(p.x), rowb + half * 64);
-          }
         }
-      };
-
-      const float* arow = acc_s + r * kAccPitch + ch * half_cols;
-      for (int c0 = 0; c0 < half_cols; c0 += 32) {
-        uint32_t v[32];
+        __syncwarp();
 #pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          const uint4 t = *reinterpret_cast<const uint4*>(arow + c0 + 4 * j);
-          v[4 * j] = t.x; v[4 * j + 1] = t.y; v[4 * j + 2] = t.z; v[4 * j + 3] = t.w;
-        }
-        process(v, c0);
+        for (int k = 0; k < 4; ++k)
+          if ((row_ok >> k) & 1u)
+            *reinterpret_cast<uint4*>(const_cast<uint8_t*>(piece_gmem(k, c, p.x, p.out_hi, p.out_lo))) =
+                *reinterpret_cast<const uint4*>(piece_smem(k));
+        __syncwarp();                                  // the staging buffer is free for the next chunk
       }
-      // the ring may take the next tile's operands: order these generic-proxy accesses before the TMA writes
-      fence_proxy_async();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&tail.ring_free_bar);
-      if (e == 0 && lane == 0) GSTAMP(unit * 4 + 3);
+      if (stamp) GSTAMP(unit * 4 + 3);
     }
   }
 }
 
-cudaError_t read_gemm_stamps(long long* host64) { return cudaMemcpyFromSymbol(host64, g_gemm_stamp, sizeof(long long) * 64); }
+cudaError_t read_gemm_stamps(long long* host128) { return cudaMemcpyFromSymbol(host128, g_gemm_stamp, sizeof(g_gemm_stamp)); }
 
 namespace {
 template <bool kSwap, int kTileN, bool kF16, int kMode>

@@ -303,9 +303,10 @@ int gp_vit_time_linears(gp_vit_handle_t h, int b, int iters, float* avg_ms, void
 /* diagnostics: SM-cycle stamps of CTA 0 of the last attention launch (synchronises the device); 32 int64 values:
  * [0] start, [1] Q/K landed, [2 + w] warpgroup w (0, 1) done with its query tiles; the other entries are not written. */
 int gp_debug_attention_timeline(long long* stamps32);
-/* same for CTA 0 of the last QKV-shaped ViT GEMM: 64 int64: [4*tile + {0: MMA start, 1: MMA done, 2: epilogue
- * start, 3: epilogue end}], [63] = kernel start. */
-int gp_debug_gemm_timeline(long long* stamps64);
+/* same for CTA 0 of the last gp_debug_gemm launch with `stamp` set: 128 int64, for the CTA's first 15 tiles
+ * [4*tile + {0: MMA start, 1: MMA done, 2: epilogue start, 3: epilogue end}] and [64 + tile] = the tile's first
+ * k-block has landed in shared memory; [63] = kernel start.  Other entries are not written. */
+int gp_debug_gemm_timeline(long long* stamps128);
 /* runs the first `num_convs` convolutions of the trunk and writes the last one's output as f32 NHWC */
 int gp_debug_ist_trunk(gp_ist_trunk_handle_t h, int n, const float* crops, int num_convs, float* activation, void* stream);
 
@@ -323,6 +324,7 @@ int gp_debug_sim_tiles(gp_handle_t h, int B, float* tiles, void* stream);
  *   swap       1: A is the 128-row operand and the outputs are written transposed, as planes [N, M]; bias is per row of A
  *   acc_scale  0 = off, else C = acc * acc_scale + bias
  *   m_dev      nullable device int32: the rows computed are min(*m_dev, M)
+ *   stamp      1: CTA 0 records the cycle timeline read by gp_debug_gemm_timeline
  * Unsupported combinations are rejected with GP_ERR_INVALID before any device is touched. */
 typedef struct gp_debug_gemm {
   int32_t M, N, K, bn, passes, mode, swap, f16;
@@ -337,6 +339,7 @@ typedef struct gp_debug_gemm {
   const uint16_t *res_hi, *res_lo;   /* residual planes, same layout as the output planes (mode 6) */
   const int32_t* m_dev;
   int32_t tokens_per_img, patches_per_img, qkv_crop_stride;
+  int32_t stamp;
 } gp_debug_gemm_t;
 int gp_debug_gemm(const gp_debug_gemm_t* g, void* stream);
 
