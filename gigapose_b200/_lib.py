@@ -65,6 +65,21 @@ class GpPredictions(C.Structure):
                 ("ransac", GpRansacOut), ("scores", C.c_void_p), ("poses", C.c_void_p)]
 
 
+class GpIcpDebug(C.Structure):
+    _fields_ = [("counts", C.c_void_p), ("sources", C.c_void_p), ("assoc", C.c_void_p), ("pose0", C.c_void_p),
+                ("iterations", C.c_void_p)]
+
+
+class GpIcpParams(C.Structure):
+    _fields_ = [("unit_per_m", C.c_float), ("min_points", C.c_int32), ("num_levels", C.c_int32),
+                ("max_iters", C.c_int32), ("rejection_scale", C.c_float), ("max_residual", C.c_float),
+                ("min_step_rad", C.c_float), ("min_step_m", C.c_float), ("debug", GpIcpDebug)]
+
+
+# gp_icp_refine statuses (GP_ICP_*)
+ICP_OK, ICP_TOO_FEW_POINTS, ICP_DEGENERATE, ICP_RESIDUAL, ICP_INVALID, ICP_LOST = 0, 1, 2, 3, 4, 5
+
+
 # every symbol include/gigapose_b200.h declares: name -> (restype, argtypes)
 SYMBOLS = {
     "gp_last_error": (C.c_char_p, []),
@@ -109,6 +124,12 @@ SYMBOLS = {
     "gp_render_templates": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p,
                                       C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
                                       C.c_float, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "gp_icp_query_sizes": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_size_t)]),
+    "gp_icp_prepare_scene": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_float, C.c_void_p,
+                                       C.c_void_p]),
+    "gp_icp_refine": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                C.c_void_p, C.c_void_p, C.POINTER(GpIcpParams), C.c_void_p, C.c_void_p, C.c_void_p,
+                                C.c_void_p, C.c_void_p, C.c_void_p]),
     "gp_ist_trunk_query_sizes":(C.c_int, [C.c_int, C.POINTER(C.c_size_t), C.POINTER(C.c_size_t)]),
     "gp_ist_trunk_create": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                       C.POINTER(C.c_void_p)]),

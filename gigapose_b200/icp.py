@@ -1,0 +1,154 @@
+"""Depth refinement of coarse poses on the GPU (row f6): every hypothesis is rendered at its pose with the frame's K
+(`gp_render_templates`), the measured depth of each frame becomes an organised target map with normals
+(`gp_icp_prepare_scene`), and one CTA per hypothesis runs the centroid shift and a point-to-plane ICP
+(`gp_icp_refine`).  csrc/depth_icp.cu's header comment states the contract; it restates MegaPose's ICPRefiner
+(src/megapose/inference/icp_refiner.py:134-287) with the deviations listed in INTEGRATION.md."""
+from __future__ import annotations
+
+import ctypes as C
+
+import torch
+
+from . import _lib
+from ._lib import GpIcpDebug, GpIcpParams, check
+from .render import _device_mesh, render_chunk
+
+STATUS_NAMES = {_lib.ICP_OK: "ok", _lib.ICP_TOO_FEW_POINTS: "too few points", _lib.ICP_DEGENERATE: "degenerate",
+                _lib.ICP_RESIDUAL: "residual above max_residual", _lib.ICP_INVALID: "invalid frame index",
+                _lib.ICP_LOST: "lost: no pairs, or fewer than 6 kept"}
+DEFAULTS = dict(unit_per_m=1000.0, min_points=1000, num_levels=4, max_iters=100, rejection_scale=2.5,
+                max_residual=0.01, min_step_rad=1e-6, min_step_m=1e-6)
+WORKSPACE_BYTES = 1 << 30          # renders + ICP scratch per chunk of hypotheses: ~20 MB per 640 x 480 hypothesis
+
+
+def _ptr(x):
+    return x.data_ptr() if x is not None else None
+
+
+def make_params(debug=None, **params) -> GpIcpParams:
+    unknown = set(params) - set(DEFAULTS)
+    if unknown:
+        raise TypeError(f"unknown ICP parameters {sorted(unknown)}")
+    p = dict(DEFAULTS, **params)
+    out = GpIcpParams(**p)
+    if debug:
+        out.debug = GpIcpDebug(**{k: _ptr(v) for k, v in debug.items()})
+    return out
+
+
+def device_meshes(meshes, device):
+    """`read_ply` dicts (or paths) -> the device tensors the renderer takes, uploaded once."""
+    from .render import read_ply
+    return [_device_mesh(read_ply(m) if isinstance(m, str) else m, device) for m in meshes]
+
+
+def render_hypotheses(meshes_dev, labels, poses, K, frame_idx, H, W, unit_per_m=1000.0):
+    """Depth [n,H,W] and boxes [n,4] of mesh labels[i] at poses[i] with K[frame_idx[i]], rendered in groups of equal
+    (object, frame); z_near = 0.1 m, Panda3D's."""
+    device = poses.device
+    n = poses.shape[0]
+    per_view = C.c_size_t()
+    check(_lib.load().gp_render_query_sizes(1, H, W, C.byref(per_view)))
+    depth = torch.empty(n, H, W, device=device)
+    boxes = torch.empty(n, 4, dtype=torch.int64, device=device)
+    lab, fr = labels.tolist(), frame_idx.tolist()
+    groups = {}
+    for i, key in enumerate(zip(lab, fr)):
+        groups.setdefault(key, []).append(i)
+    chunk = max(1, min(n, WORKSPACE_BYTES // 2 // (per_view.value + 16 * H * W)))
+    ws = torch.empty(chunk * per_view.value, dtype=torch.uint8, device=device)
+    rgba = torch.empty(chunk, 4, H, W, device=device)
+    for (o, f), idx in groups.items():
+        for s in range(0, len(idx), chunk):
+            sel = torch.tensor(idx[s:s + chunk], device=device)
+            m = len(sel)
+            d, b = torch.empty(m, H, W, device=device), torch.empty(m, 4, dtype=torch.int64, device=device)
+            render_chunk(meshes_dev[o], poses[sel].contiguous(), K[f].contiguous(), H, W, 0.1 * unit_per_m, ws,
+                         rgba[:m], d, b)
+            depth[sel], boxes[sel] = d, b
+    return depth, boxes
+
+
+def prepare_scene(depth, K, workspace, unit_per_m=1000.0):
+    F, H, W = depth.shape
+    check(_lib.load().gp_icp_prepare_scene(F, H, W, depth.data_ptr(), K.data_ptr(), float(unit_per_m),
+                                           workspace.data_ptr(), torch.cuda.current_stream(depth.device).cuda_stream))
+
+
+def workspace_bytes(n_frames, n_hyp, H, W):
+    b = C.c_size_t()
+    check(_lib.load().gp_icp_query_sizes(n_frames, n_hyp, H, W, C.byref(b)))
+    return b.value
+
+
+def refine_rendered(depth, K, frame_idx, rendered, boxes, poses, masks, workspace, debug=None, **params):
+    """gp_icp_refine over n hypotheses whose scene is already in `workspace` -> poses, status, residual, fitness."""
+    F, H, W = depth.shape
+    n = poses.shape[0]
+    dev = poses.device
+    out = torch.empty(n, 4, 4, device=dev)
+    status = torch.empty(n, dtype=torch.int32, device=dev)
+    residual = torch.empty(n, device=dev)
+    fitness = torch.empty(n, device=dev)
+    p = make_params(debug, **params)
+    check(_lib.load().gp_icp_refine(F, n, H, W, frame_idx.data_ptr(), _ptr(masks), rendered.data_ptr(), boxes.data_ptr(),
+                                    poses.data_ptr(), K.data_ptr(), C.byref(p), out.data_ptr(), status.data_ptr(),
+                                    residual.data_ptr(), fitness.data_ptr(), workspace.data_ptr(),
+                                    torch.cuda.current_stream(dev).cuda_stream))
+    return out, status, residual, fitness
+
+
+@torch.no_grad()
+def refine_icp(meshes_dev, labels, poses, depth, K, frame_idx, masks=None, **params):
+    """Refines n hypotheses against the measured depth.
+
+    meshes_dev  list of device meshes (`device_meshes`), indexed by labels [n] (0-based);
+    poses       [n,4,4] coarse object -> camera poses, in the depth unit;
+    depth       [F,H,W] measured depth (0 = missing), K [F,3,3] full-image intrinsics, frame_idx [n] frame of each;
+    masks       None (the reference's threshold rule) or [n,H,W] full-frame detection masks;
+    params      see DEFAULTS (unit_per_m = 1000 for mm).
+    -> (poses [n,4,4], status [n] i32 (STATUS_NAMES), residual [n], fitness [n]) on the device; a pose whose status is
+    not 0 is its input pose bit for bit."""
+    device = poses.device
+    if device.type != "cuda":
+        raise _lib.GigaPoseNativeError("refine_icp runs on CUDA devices only (no CPU fallback)")
+    upm = float(params.get("unit_per_m", DEFAULTS["unit_per_m"]))
+    poses = poses.to(device, torch.float32).reshape(-1, 4, 4).contiguous()
+    depth = torch.as_tensor(depth).to(device, torch.float32).contiguous()
+    if depth.dim() == 2:
+        depth = depth[None]
+    F, H, W = depth.shape
+    K = torch.as_tensor(K).to(device, torch.float32)
+    if tuple(K.shape) not in ((3, 3), (1, 3, 3), (F, 3, 3)):
+        raise ValueError(f"K must be [3,3] or one full-image K per frame [{F},3,3], got {tuple(K.shape)}")
+    K = K.reshape(-1, 3, 3).expand(F, 3, 3).contiguous()
+    n = poses.shape[0]
+    labels = torch.as_tensor(labels).reshape(-1).to("cpu", torch.int64)
+    frame_idx = torch.as_tensor(frame_idx).reshape(-1).to("cpu", torch.int64)
+    if labels.shape[0] != n or frame_idx.shape[0] != n:
+        raise ValueError("labels and frame_idx need one entry per pose")
+    if n and (int(labels.min()) < 0 or int(labels.max()) >= len(meshes_dev)):
+        raise ValueError(f"labels outside [0, {len(meshes_dev)})")
+    if n and (int(frame_idx.min()) < 0 or int(frame_idx.max()) >= F):
+        raise ValueError(f"frame_idx outside [0, {F})")
+    if masks is not None:
+        masks = torch.as_tensor(masks).to(device).reshape(n, H, W).to(torch.uint8).contiguous()
+    out = poses.clone()
+    status = torch.empty(n, dtype=torch.int32, device=device)
+    residual = torch.empty(n, device=device)
+    fitness = torch.empty(n, device=device)
+    if n == 0:
+        return out, status, residual, fitness
+    scene = workspace_bytes(F, 0, H, W)
+    per_hyp = workspace_bytes(F, 1, H, W) - scene
+    chunk = max(1, min(n, WORKSPACE_BYTES // (per_hyp + 52 * H * W)))
+    ws = torch.empty(scene + chunk * per_hyp, dtype=torch.uint8, device=device)
+    prepare_scene(depth, K, ws, upm)
+    fi = frame_idx.to(device, torch.int32)
+    for s in range(0, n, chunk):
+        sl = slice(s, min(n, s + chunk))
+        rendered, boxes = render_hypotheses(meshes_dev, labels[sl], poses[sl], K, frame_idx[sl], H, W, upm)
+        o = refine_rendered(depth, K, fi[sl].contiguous(), rendered, boxes, poses[sl],
+                            None if masks is None else masks[sl], ws, **params)
+        out[sl], status[sl], residual[sl], fitness[sl] = o
+    return out, status, residual, fitness

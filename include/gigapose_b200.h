@@ -290,6 +290,56 @@ int gp_render_templates(int n_views, int height, int width, int num_vertices, co
                         int tex_h, int tex_w, const float* constant_color, const float* poses, const float* K,
                         float z_near, void* workspace, float* rgba, float* depth, int64_t* boxes, void* stream);
 
+/* --- row f6: depth refinement of the coarse poses (MegaPose's ICPRefiner, src/megapose/inference/icp_refiner.py:134-287,
+ * with a GPU point-to-plane ICP in place of OpenCV's ppf_match_3d_ICP).  The full contract is the header comment of
+ * gigapose_b200/csrc/depth_icp.cu.  Needs no handle. ------------------------------------------------------------- */
+#define GP_ICP_OK 0               /* refined pose accepted */
+#define GP_ICP_TOO_FEW_POINTS 1   /* fewer than min_points targets or sources: T0 returned */
+#define GP_ICP_DEGENERATE 2       /* singular point-to-plane system (e.g. a planar object): T0 returned */
+#define GP_ICP_RESIDUAL 3         /* converged with residual > max_residual: T0 returned */
+#define GP_ICP_INVALID 4          /* frame_idx outside [0, n_frames): T0 returned */
+#define GP_ICP_LOST 5             /* an iteration found no pair, or kept fewer than 6: T0 returned */
+
+typedef struct gp_icp_debug {    /* every field nullable; test and timing hooks */
+  int32_t* counts;               /* [n_hyp,2] number of targets, sources */
+  int32_t* sources;              /* [n_hyp,H*W] compacted source pixel indices (row-major), first `sources` entries */
+  int32_t* assoc;                /* [n_hyp,H*W] last level-0 iteration, per level-0 source: the target pixel index of a
+                                    kept pair, -2 - index of a rejected one, -1 for no pair */
+  float* pose0;                  /* [n_hyp,3,4] the correction after the centroid shift, before the first iteration */
+  int32_t* iterations;           /* [n_hyp,num_levels] iterations run per level (index = level); not written for
+                                    levels that were not reached */
+} gp_icp_debug_t;
+
+typedef struct gp_icp_params {
+  float unit_per_m;              /* depth / translation units per metre (1000 for BOP's mm) */
+  int32_t min_points;            /* n_min_points, 1000 (icp_refiner.py:178) */
+  int32_t num_levels;            /* 4 (numLevels) */
+  int32_t max_iters;             /* per level, 100 */
+  float rejection_scale;         /* pairs farther than this x the median distance are dropped, 2.5 */
+  float max_residual;            /* metres, 0.01: above it the coarse pose is kept */
+  float min_step_rad;            /* a level stops after a step below both, 1e-6 rad ... */
+  float min_step_m;              /* ... and 1e-6 m */
+  gp_icp_debug_t debug;
+} gp_icp_params_t;
+
+/* Workspace bytes for n_frames frames and n_hyp hypotheses of height x width (17 <= sides <= 8192): 36 B per frame
+ * pixel for the scene, 12 B per hypothesis pixel. */
+int gp_icp_query_sizes(int n_frames, int n_hyp, int height, int width, size_t* workspace_bytes);
+/* Per frame: depth f32 [n_frames,H,W] (0 = missing), K f32 [n_frames,3,3] full-image intrinsics.  Smooths the depth
+ * and writes the organised target map; after the call the workspace starts with it, f32 [n_frames,H,W,6] = (x, y, z,
+ * normal), z = 0 outside (0.2, 5) m. */
+int gp_icp_prepare_scene(int n_frames, int height, int width, const float* depth, const float* K, float unit_per_m,
+                         void* workspace, void* stream);
+/* Per hypothesis, after gp_icp_prepare_scene on the same workspace: frame_idx i32 [n_hyp], masks u8 [n_hyp,H,W]
+ * full-frame detection masks or NULL (threshold rule), rendered_depth f32 [n_hyp,H,W] and boxes i64 [n_hyp,4] from
+ * gp_render_templates at T0 f32 [n_hyp,4,4] with the frame's K (the same K pointer as the scene).  Outputs: out_poses
+ * f32 [n_hyp,4,4] (T0 bit for bit unless the status is GP_ICP_OK), out_status i32, out_residual f32 (RMS
+ * point-to-plane distance, depth unit; -1 when not reached), out_fitness f32 (kept pairs / level-0 sources). */
+int gp_icp_refine(int n_frames, int n_hyp, int height, int width, const int32_t* frame_idx, const uint8_t* masks,
+                  const float* rendered_depth, const int64_t* boxes, const float* T0, const float* K,
+                  const gp_icp_params_t* params, float* out_poses, int32_t* out_status, float* out_residual,
+                  float* out_fitness, void* workspace, void* stream);
+
 /* --- diagnostics ----------------------------------------------------------------------------------------- */
 /* number of kernels this library has launched since load (all handles); used for bench.py's `gpu_launches` */
 uint64_t gp_launch_count(void);

@@ -269,6 +269,61 @@ class GigaPose(LightningModule):
         logger.info(f"Onboarded {dataset_name}: {n_obj} objects x {T} templates, {self.onboarding_s_per_object:.3f} s/object")
         return eng
 
+    # ------------------------------------------------------------------ row f6: depth refinement (icp_refiner.py:134-287)
+    def attach_meshes(self, dataset_name, meshes):
+        """Uploads the CAD meshes of `dataset_name` once for `refine_depth`: PLY paths or `read_ply` dicts, in object
+        order (label 1 is meshes[0]), vertices in the unit of the pose translations."""
+        from gigapose_b200.icp import device_meshes
+        if not hasattr(self, "meshes"):
+            self.meshes = {}
+        self.meshes[dataset_name] = device_meshes(meshes, self.device if self.device.type == "cuda" else "cuda")
+
+    @torch.no_grad()
+    def refine_depth(self, dataset_name, predictions, depth, frame_idx=None, masks=None, hypotheses=1, *, K=None,
+                     **params):
+        """MegaPose's ICPRefiner.refine_poses on the output of `retrieve()`: the first `hypotheses` of the k poses of every
+        detection are rendered and refined against the measured depth (gigapose_b200.icp.refine_icp).
+
+        depth [F,H,W] (or [H,W]) measured depth in the unit of the poses, 0 = missing; frame_idx [B] frame of each
+        detection (default: the `batch_im_id` column, or 0 for a single frame); masks None (threshold rule) or [B,H,W]
+        full-frame detection masks; K, keyword only and required, the frames' full-image intrinsics [F,3,3] (or one
+        [3,3] for all): `retrieve()`'s output does not carry them, and the batch's per-detection `tar_K` [B,3,3] is
+        indexed by detection, not by frame (pass `tar_K[i]` of one detection i per frame); params as
+        gigapose_b200.icp.DEFAULTS.  Returns a new collection: `pred_poses` replaced where the
+        refinement was accepted (same order, nothing re-sorted), `poses_input` the coarse poses, and `icp_status`,
+        `icp_residual`, `icp_fitness` [B,hypotheses]."""
+        from gigapose_b200.icp import refine_icp
+        if K is None:
+            raise TypeError("refine_depth needs K=, the frames' full-image intrinsics [F,3,3] or [3,3]")
+        meshes = self.meshes[dataset_name]
+        poses = predictions.pred_poses
+        B, k = poses.shape[:2]
+        h = max(1, min(int(hypotheses), k))
+        depth = torch.as_tensor(depth)
+        n_frames = 1 if depth.dim() == 2 else depth.shape[0]
+        if frame_idx is None:
+            if "batch_im_id" in predictions.infos:
+                frame_idx = np.asarray(predictions.infos.batch_im_id, np.int64)
+            elif n_frames == 1:
+                frame_idx = np.zeros(B, np.int64)
+            else:
+                raise ValueError("frame_idx is needed when depth holds several frames")
+        frame_idx = np.asarray(torch.as_tensor(frame_idx).cpu()).reshape(-1)
+        labels = object_indices(predictions.infos, len(meshes))
+        if masks is not None:
+            masks = torch.as_tensor(masks).to(poses.device).repeat_interleave(h, 0)
+        out, status, residual, fitness = refine_icp(meshes, np.repeat(labels, h), poses[:, :h].reshape(-1, 4, 4),
+                                                    depth, K, np.repeat(frame_idx, h), masks, **params)
+        refined = predictions.clone()
+        refined.register_tensor("poses_input", poses.clone())
+        new = poses.clone()
+        new[:, :h] = out.reshape(B, h, 4, 4)
+        refined.register_tensor("pred_poses", new)
+        refined.register_tensor("icp_status", status.reshape(B, h))
+        refined.register_tensor("icp_residual", residual.reshape(B, h))
+        refined.register_tensor("icp_fitness", fitness.reshape(B, h))
+        return refined
+
     # ------------------------------------------------------------------ localisation filter + writer (gigaPose.py:400-449)
     def filter_and_save(self, predictions, test_list, time, save_path, keep_only_testing_instances=True):
         labels = np.asarray(predictions.infos.label).astype(np.int32)
