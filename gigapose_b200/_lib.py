@@ -140,6 +140,7 @@ SYMBOLS = {
     "gp_debug_gemm": (C.c_int, [C.POINTER(GpDebugGemm), C.c_void_p]),
     "gp_debug_attention": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                      C.c_void_p]),
+    "gp_debug_layernorm": (C.c_int, [C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "gp_normalize_patch_tokens": (C.c_int, [C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
     "gp_vit_time_linears": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.POINTER(C.c_float), C.c_void_p]),
     "gp_time_sim_kernel": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.POINTER(C.c_float), C.c_void_p]),

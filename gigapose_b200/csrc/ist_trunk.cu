@@ -174,12 +174,13 @@ void carve_workspace(Carver& c, int max_crops, gp_ist_trunk_context* h) {
   if (h) { h->stem.hi = a; h->stem.lo = l; }
 }
 
-int run(gp_ist_trunk_context* h, int n, const float* crops, float* feat, int stop_after, float* dump, cudaStream_t s) {
+// Runs the resize and the first `last` convolutions; `dump` (if set) receives the merged output planes of convolution
+// `last` (last = 0: the zero-bordered resized-crop planes).
+int run(gp_ist_trunk_context* h, int n, const float* crops, float* feat, int last, float* dump, cudaStream_t s) {
   resize_pad_kernel<<<(n * kRes * kRes + 255) / 256, 256, 0, s>>>(crops, n, reinterpret_cast<uint2*>(h->stem.hi),
                                                                   reinterpret_cast<uint2*>(h->stem.lo));
   GPI_CUDA(cudaGetLastError());
   int launched = 1;
-  const int last = stop_after > 0 && stop_after < (int)h->convs.size() ? stop_after : (int)h->convs.size();
   for (int i = 0; i < last; ++i) {
     const Conv& c = h->convs[i];
     gp::GemmParams g{};
@@ -200,12 +201,16 @@ int run(gp_ist_trunk_context* h, int n, const float* crops, float* feat, int sto
     ++launched;
   }
   if (dump) {
-    const Conv& c = h->convs[last - 1];
-    if (c.out_buf < 0) return gp_internal_fail(GP_ERR_INVALID, "the last convolution writes `feat` directly; nothing to dump");
-    const long long cnt = (long long)n * c.hout * c.hout * c.cout;
+    const Planes* src = &h->stem;
+    long long cnt = (long long)n * kPadRows * kPadCols * 4;
+    if (last > 0) {
+      const Conv& c = h->convs[last - 1];
+      if (c.out_buf < 0) return gp_internal_fail(GP_ERR_INVALID, "the last convolution writes `feat` directly; nothing to dump");
+      src = &h->act[c.out_buf];
+      cnt = (long long)n * c.hout * c.hout * c.cout;
+    }
     merge_planes_kernel<<<(unsigned)((cnt + 255) / 256), 256, 0, s>>>(
-        reinterpret_cast<const __nv_bfloat16*>(h->act[c.out_buf].hi), reinterpret_cast<const __nv_bfloat16*>(h->act[c.out_buf].lo),
-        cnt, dump);
+        reinterpret_cast<const __nv_bfloat16*>(src->hi), reinterpret_cast<const __nv_bfloat16*>(src->lo), cnt, dump);
     GPI_CUDA(cudaGetLastError());
     ++launched;
   }
@@ -304,13 +309,13 @@ int gp_ist_trunk_destroy(gp_ist_trunk_handle_t h) {
 int gp_ist_trunk_forward(gp_ist_trunk_handle_t h, int n, const float* crops, float* feat, void* stream) {
   if (!h || !crops || !feat) return gp_internal_fail(GP_ERR_INVALID, "null argument");
   if (n < 1 || n > h->max_crops) return gp_internal_fail(GP_ERR_INVALID, "batch %d outside [1, %d]", n, h->max_crops);
-  return run(h, n, crops, feat, 0, nullptr, static_cast<cudaStream_t>(stream));
+  return run(h, n, crops, feat, kNumConvs, nullptr, static_cast<cudaStream_t>(stream));
 }
 
 int gp_debug_ist_trunk(gp_ist_trunk_handle_t h, int n, const float* crops, int num_convs, float* activation, void* stream) {
   if (!h || !crops || !activation) return gp_internal_fail(GP_ERR_INVALID, "null argument");
   if (n < 1 || n > h->max_crops) return gp_internal_fail(GP_ERR_INVALID, "batch %d outside [1, %d]", n, h->max_crops);
-  if (num_convs < 1 || num_convs >= kNumConvs) return gp_internal_fail(GP_ERR_INVALID, "num_convs outside [1, %d)", kNumConvs);
+  if (num_convs < 0 || num_convs >= kNumConvs) return gp_internal_fail(GP_ERR_INVALID, "num_convs outside [0, %d)", kNumConvs);
   return run(h, n, crops, nullptr, num_convs, activation, static_cast<cudaStream_t>(stream));
 }
 

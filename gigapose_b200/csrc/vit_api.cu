@@ -21,6 +21,7 @@ extern int gp_internal_make_map_ex(CUtensorMap* map, void* ptr, uint64_t rows, u
 namespace {
 
 constexpr int kDim = 1024, kQkv = 3072, kMlp = 4096, kTok = 257, kPatchK = 588, kPatchKPad = 608;
+constexpr float kLayerNormEps = 1e-6f;          // DINOv2's norm layers (nn.LayerNorm(eps=1e-6)); gp_debug_layernorm uses it too
 constexpr size_t kAlign = 1024;
 inline size_t up(size_t x) { return (x + kAlign - 1) / kAlign * kAlign; }
 
@@ -233,6 +234,15 @@ int gp_debug_attention(int b, int crop_stride, int passes, const uint16_t* qkv_h
   return GP_OK;
 }
 
+int gp_debug_layernorm(int M, const float* x, const float* w, const float* b, uint16_t* out_hi, uint16_t* out_lo,
+                       void* stream) {
+  if (!x || !w || !b || !out_hi || !out_lo) return gp_internal_fail(GP_ERR_INVALID, "null argument");
+  if (M < 1) return gp_internal_fail(GP_ERR_INVALID, "M must be >= 1");
+  GPV_CUDA(gp::launch_layernorm_planes(x, M, w, b, kLayerNormEps, out_hi, out_lo, static_cast<cudaStream_t>(stream)));
+  gp_internal_count_launches(1);
+  return GP_OK;
+}
+
 int gp_vit_destroy(gp_vit_handle_t h) {
   delete h;
   return GP_OK;
@@ -303,7 +313,7 @@ int gp_vit_forward(gp_vit_handle_t h, int b, const float* img, float* x_prenorm,
   };
   for (int i = 0; i < h->depth; ++i) {
     const BlockW& B = h->blocks[i];
-    GPV_CUDA(gp::launch_layernorm_planes(h->x, M, B.n1w, B.n1b, 1e-6f, h->ln.hi, h->ln.lo, s));
+    GPV_CUDA(gp::launch_layernorm_planes(h->x, M, B.n1w, B.n1b, kLayerNormEps, h->ln.hi, h->ln.lo, s));
     g = gp::GemmParams{}; g.passes = h->passes;
     g.M = M; g.N = kQkv; g.K = kDim; g.mode = gp::GEMM_QKV_HEADS; g.bias = B.qkv_b; g.out_hi = h->qkv.hi; g.out_lo = h->qkv.lo;
     g.tokens_per_img = kTok; g.qkv_crop_stride = h->max_crops;
@@ -313,7 +323,7 @@ int gp_vit_forward(gp_vit_handle_t h, int b, const float* img, float* x_prenorm,
     g = gp::GemmParams{}; g.passes = h->passes;
     g.M = M; g.N = kDim; g.K = kDim; g.mode = gp::GEMM_SCALE_RESIDUAL; g.bias = B.proj_b; g.gamma = B.ls1; g.x = h->x;
     GPV_CUDA(linear(h->attn, B.proj, g));
-    GPV_CUDA(gp::launch_layernorm_planes(h->x, M, B.n2w, B.n2b, 1e-6f, h->ln.hi, h->ln.lo, s));
+    GPV_CUDA(gp::launch_layernorm_planes(h->x, M, B.n2w, B.n2b, kLayerNormEps, h->ln.hi, h->ln.lo, s));
     g = gp::GemmParams{}; g.passes = h->passes;
     g.M = M; g.N = kMlp; g.K = kDim; g.mode = gp::GEMM_PLANES_GELU; g.bias = B.fc1_b; g.out_hi = h->hid.hi; g.out_lo = h->hid.lo;
     GPV_CUDA(linear(h->ln, B.fc1, g));

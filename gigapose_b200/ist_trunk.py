@@ -113,7 +113,8 @@ class NativeISTTrunk:
 
     @torch.no_grad()
     def activation_after(self, x: torch.Tensor, num_convs: int) -> torch.Tensor:
-        """Test hook: NHWC output of the `num_convs`-th convolution (execution order) as fp32 [n,h,w,c]."""
+        """Test hook: NHWC output of the `num_convs`-th convolution (execution order) as fp32 [n,h,w,c]; num_convs = 0
+        gives the stem's input, the resized crops with their zero border, as fp32 [n,262,264,4]."""
         shapes = []
         h = 128
         shapes.append((h, 128))
@@ -124,10 +125,14 @@ class NativeISTTrunk:
                     shapes += [(h, d), (h, d), (h, d)]
                 else:
                     shapes += [(h, d), (h, d)]
-        hh, cc = shapes[num_convs - 1]
         x = x.to(self.device, dtype=torch.float32).contiguous()
         assert x.shape[0] <= self.max_crops
-        out = torch.empty(x.shape[0], hh, hh, cc, device=self.device)
+        if num_convs == 0:
+            shape = (262, 264, 4)
+        else:
+            hh, cc = shapes[num_convs - 1]
+            shape = (hh, hh, cc)
+        out = torch.empty(x.shape[0], *shape, device=self.device)
         check(self.lib.gp_debug_ist_trunk(self._h, x.shape[0], x.data_ptr(), num_convs, out.data_ptr(),
                                           torch.cuda.current_stream(self.device).cuda_stream))
         return out

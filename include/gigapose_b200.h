@@ -357,7 +357,10 @@ int gp_debug_attention_timeline(long long* stamps32);
  * [4*tile + {0: MMA start, 1: MMA done, 2: epilogue start, 3: epilogue end}] and [64 + tile] = the tile's first
  * k-block has landed in shared memory; [63] = kernel start.  Other entries are not written. */
 int gp_debug_gemm_timeline(long long* stamps128);
-/* runs the first `num_convs` convolutions of the trunk and writes the last one's output as f32 NHWC */
+/* runs the first `num_convs` convolutions of the trunk (0 <= num_convs < GP_IST_TRUNK_NUM_CONVS) and writes the last
+ * one's output planes, merged (hi + lo), as f32 NHWC [n, h, w, c].  num_convs = 0 writes the stem's input instead: the
+ * bilinear-resized crops, merged, as f32 [n, 262, 264, 4] -- pixel (y, x) of the 256 x 256 crop at row y + 3, column
+ * x + 4, channels 0-2; the 3-row / 4-column border and channel 3 are zero (the stem convolution's padding). */
 int gp_debug_ist_trunk(gp_ist_trunk_handle_t h, int n, const float* crops, int num_convs, float* activation, void* stream);
 
 /* test hook: runs the similarity kernel and additionally dumps the raw fp32 similarity tiles, laid out
@@ -398,6 +401,11 @@ int gp_debug_gemm(const gp_debug_gemm_t* g, void* stream);
  * out_hi / out_lo: bf16 planes [b * 257, 1024] (token rows, head h in columns [64 h, 64 h + 64)).  passes: 3 or 1. */
 int gp_debug_attention(int b, int crop_stride, int passes, const uint16_t* qkv_hi, const uint16_t* qkv_lo, uint16_t* out_hi,
                        uint16_t* out_lo, void* stream);
+
+/* test hook: the LayerNorm kernel of the ViT alone, with the eps gp_vit_forward uses (1e-6).  x f32 [M, 1024] rows,
+ * w / b f32 [1024]; out_hi / out_lo: bf16 planes [M, 1024] of (x - mean) / sqrt(var + eps) * w + b.  M >= 1. */
+int gp_debug_layernorm(int M, const float* x, const float* w, const float* b, uint16_t* out_hi, uint16_t* out_lo,
+                       void* stream);
 
 #ifdef __cplusplus
 }

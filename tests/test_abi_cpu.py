@@ -125,8 +125,8 @@ def test_num_templates_beyond_the_topk_shared_memory_is_rejected(lib):
 
 
 def test_debug_kernel_entries_reject_bad_arguments_without_a_gpu(lib):
-    """gp_debug_gemm / gp_debug_attention check their arguments before they touch a device: an unsupported GEMM
-    configuration fails with GP_ERR_INVALID and says why."""
+    """gp_debug_gemm / gp_debug_attention / gp_debug_layernorm check their arguments before they touch a device: an
+    unsupported GEMM configuration fails with GP_ERR_INVALID and says why."""
     fake = 1 << 20                                   # never dereferenced: every call below fails validation first
 
     def gemm(**kw):
@@ -170,3 +170,8 @@ def test_debug_kernel_entries_reject_bad_arguments_without_a_gpu(lib):
     assert att(1, 5, 2) == -1 and b"passes" in lib.gp_last_error()
     for null in ("hi", "lo", "oh", "ol"):
         assert att(1, 5, 3, **{null: None}) == -1 and b"null" in lib.gp_last_error()
+    ln = lambda M, x=fake, w=fake, b=fake, oh=fake, ol=fake: lib.gp_debug_layernorm(M, x, w, b, oh, ol, None)
+    for null in ("x", "w", "b", "oh", "ol"):
+        assert ln(8, **{null: None}) == -1 and b"null" in lib.gp_last_error()
+    for M in (0, -5):
+        assert ln(M) == -1 and b"M must be" in lib.gp_last_error()
