@@ -65,9 +65,17 @@ class GpPredictions(C.Structure):
                 ("ransac", GpRansacOut), ("scores", C.c_void_p), ("poses", C.c_void_p)]
 
 
+class GpIcpTrace(C.Structure):
+    """gp_icp_trace_t: one ICP iteration of one hypothesis (456 bytes; np.dtype(GpIcpTrace) reads an array of them)."""
+    _fields_ = [("level", C.c_int32), ("iteration", C.c_int32), ("n", C.c_int32), ("found", C.c_int32),
+                ("kept", C.c_int32), ("done", C.c_int32), ("median_bits", C.c_uint32), ("reserved", C.c_int32),
+                ("Tf", C.c_float * 12), ("sums", C.c_double * 29), ("xi", C.c_double * 6), ("dT", C.c_double * 12)]
+
+
 class GpIcpDebug(C.Structure):
     _fields_ = [("counts", C.c_void_p), ("sources", C.c_void_p), ("assoc", C.c_void_p), ("pose0", C.c_void_p),
-                ("iterations", C.c_void_p)]
+                ("iterations", C.c_void_p), ("trace", C.c_void_p), ("trace_capacity", C.c_int32),
+                ("trace_count", C.c_void_p)]
 
 
 class GpIcpParams(C.Structure):
@@ -130,6 +138,7 @@ SYMBOLS = {
     "gp_icp_refine": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                 C.c_void_p, C.c_void_p, C.POINTER(GpIcpParams), C.c_void_p, C.c_void_p, C.c_void_p,
                                 C.c_void_p, C.c_void_p, C.c_void_p]),
+    "gp_debug_icp_select": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
     "gp_ist_trunk_query_sizes":(C.c_int, [C.c_int, C.POINTER(C.c_size_t), C.POINTER(C.c_size_t)]),
     "gp_ist_trunk_create": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                       C.POINTER(C.c_void_p)]),

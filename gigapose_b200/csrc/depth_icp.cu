@@ -42,6 +42,11 @@
 //
 // Layout: three scene kernels (vertical pass, horizontal pass, normals) over all frames; one persistent CTA per
 // hypothesis runs stages 2-6 without host synchronisation.  A hypothesis' result depends on its own inputs only.
+//
+// Debug hooks (tests/test_gpu_icp_solver.py): with debug.trace set, thread 0 writes one gp_icp_trace_t per iteration
+// (the fp32 transform it associated with, the counts, the median, the 29 fp64 sums, the step and the correction after
+// it), so that each step can be checked against an fp64 reference started from the kernel's own state; the outputs are
+// the same with and without it.  gp_debug_icp_select runs the median's radix_select alone.
 #include "../../include/gigapose_b200.h"
 #include "gigapose_kernels.h"
 
@@ -198,6 +203,40 @@ __device__ __forceinline__ int block_rank(bool flag, int* warp_counts, int* tota
   return before + __popc(ballot & ((1u << lane) - 1u));
 }
 
+struct SelectShared {      // scratch of radix_select
+  int hist[256];
+  unsigned prefix;
+  int rank;
+};
+
+// Exact select over the float bits of n distances (kNoPair entries are skipped): every thread of the CTA calls it with
+// the same arguments and gets the bits of the element of rank `rank` (0-based, ascending) among the others.  Radix
+// select, 8 bits per pass from the top byte; for non-negative floats the bit order is the value order.  `rank` must be
+// below the number of entries that are not kNoPair.
+__device__ unsigned radix_select(const unsigned* bits, int n, int rank, SelectShared& s) {
+  const int tid = threadIdx.x;
+  if (tid == 0) { s.prefix = 0u; s.rank = rank; }
+  for (int pass = 3; pass >= 0; --pass) {
+    if (tid < 256) s.hist[tid] = 0;
+    __syncthreads();
+    const unsigned hi_mask = pass == 3 ? 0u : ~0u << (8 * (pass + 1));
+    const unsigned prefix = s.prefix;
+    for (int i = tid; i < n; i += kThreads) {
+      const unsigned d = bits[i];
+      if (d != kNoPair && (d & hi_mask) == prefix) atomicAdd(&s.hist[(d >> (8 * pass)) & 255u], 1);
+    }
+    __syncthreads();
+    if (tid == 0) {
+      int r = s.rank, b = 0;
+      while (b < 255 && r >= s.hist[b]) { r -= s.hist[b]; ++b; }
+      s.rank = r;
+      s.prefix = prefix | ((unsigned)b << (8 * pass));
+    }
+    __syncthreads();
+  }
+  return s.prefix;
+}
+
 struct Shared {
   double red_warp[kWarps * kAcc];
   double red[kAcc];
@@ -205,13 +244,26 @@ struct Shared {
   double residual, fitness;
   float Tf[12];
   float K[4];             // fx, fy, cx, cy
-  int hist[256];
+  SelectShared sel;
   int warp_counts[kWarps];
-  unsigned prefix;
-  int rank;
   int done;               // 0 running, 1 level converged, 2 degenerate, 3 lost
   int box[4];
 };
+
+// debug trace: record `rec` of hypothesis h (thread 0 only); records past the capacity are counted, not written
+__device__ void trace_write(const gp_icp_debug_t& d, int h, int rec, int level, int it, int n, int found, unsigned median,
+                            const Shared& sh, bool have_sums, const double* xi) {
+  if (rec < d.trace_capacity) {
+    gp_icp_trace_t& t = d.trace[(size_t)h * d.trace_capacity + rec];
+    t.level = level; t.iteration = it; t.n = n; t.found = found;
+    t.kept = have_sums ? (int32_t)sh.red[28] : 0;
+    t.done = sh.done; t.median_bits = median; t.reserved = 0;
+    for (int k = 0; k < 12; ++k) { t.Tf[k] = sh.Tf[k]; t.dT[k] = sh.dT[k]; }
+    for (int k = 0; k < kAcc; ++k) t.sums[k] = have_sums ? sh.red[k] : 0.0;
+    for (int k = 0; k < 6; ++k) t.xi[k] = xi[k];
+  }
+  d.trace_count[h] = rec + 1;
+}
 
 __device__ __forceinline__ void rodrigues(const double w[3], double R[9]) {
   const double th = sqrt(w[0] * w[0] + w[1] * w[1] + w[2] * w[2]);
@@ -233,6 +285,9 @@ icp_kernel(int n_frames, int H, int W, const int32_t* __restrict__ frame_idx, co
   __shared__ Shared sh;
   const int h = blockIdx.x, tid = threadIdx.x;
   const size_t plane = (size_t)H * W;
+  const bool trace = p.debug.trace != nullptr;
+  int n_rec = 0;                                       // trace records of this hypothesis (thread 0)
+  if (tid == 0 && p.debug.trace_count) p.debug.trace_count[h] = 0;
   const float* t0 = T0 + 16 * (size_t)h;
   const float upm = p.unit_per_m;
   float* po = out_pose + 16 * (size_t)h;
@@ -360,34 +415,21 @@ icp_kernel(int n_frames, int H, int W, const int32_t* __restrict__ frame_idx, co
         wk.tgt[i] = bi;
         found += bi >= 0;
       }
-      // exact median: radix select of rank (m - 1) / 2 over the float bits, 8 bits per pass
-      {
-        int total;
-        double m_[1] = {(double)found};
-        block_sum(m_, sh.red_warp, sh.red);
-        total = (int)sh.red[0];
-        if (tid == 0) { sh.prefix = 0u; sh.rank = (total - 1) / 2; }
-        if (total == 0) { status = GP_ICP_LOST; break; }
-        for (int pass = 3; pass >= 0; --pass) {
-          if (tid < 256) sh.hist[tid] = 0;
-          __syncthreads();
-          const unsigned hi_mask = pass == 3 ? 0u : ~0u << (8 * (pass + 1));
-          const unsigned prefix = sh.prefix;
-          for (int i = tid; i < n; i += kThreads) {
-            const unsigned d = wk.dist[i];
-            if (d != kNoPair && (d & hi_mask) == prefix) atomicAdd(&sh.hist[(d >> (8 * pass)) & 255u], 1);
-          }
-          __syncthreads();
-          if (tid == 0) {
-            int r = sh.rank, b = 0;
-            while (b < 255 && r >= sh.hist[b]) { r -= sh.hist[b]; ++b; }
-            sh.rank = r;
-            sh.prefix = prefix | ((unsigned)b << (8 * pass));
-          }
-          __syncthreads();
+      // exact median: the element of rank (m - 1) / 2 of the m pair distances
+      double m_[1] = {(double)found};
+      block_sum(m_, sh.red_warp, sh.red);
+      const int total = (int)sh.red[0];
+      if (total == 0) {
+        if (trace && tid == 0) {
+          const double zero[6] = {0, 0, 0, 0, 0, 0};
+          sh.done = 3;
+          trace_write(p.debug, h, n_rec++, level, it, n, 0, kNoPair, sh, false, zero);
         }
+        status = GP_ICP_LOST;
+        break;
       }
-      const float gate = __fmul_rn(p.rejection_scale, __uint_as_float(sh.prefix));
+      const unsigned median = radix_select(wk.dist, n, (total - 1) / 2, sh.sel);
+      const float gate = __fmul_rn(p.rejection_scale, __uint_as_float(median));
       // normal equations
       double a[kAcc];
 #pragma unroll
@@ -446,12 +488,13 @@ icp_kernel(int n_frames, int H, int W, const int32_t* __restrict__ frame_idx, co
             A[r][c] = s / A[c][c];
           }
         }
+        double xi[6] = {0, 0, 0, 0, 0, 0};
         if (kept < 6.0) {
           sh.done = 3;
         } else if (!ok) {
           sh.done = 2;
         } else {
-          double y[6], xi[6];
+          double y[6];
           for (int c = 0; c < 6; ++c) {
             double s = b[c];
             for (int e = 0; e < c; ++e) s -= A[c][e] * y[e];
@@ -474,6 +517,7 @@ icp_kernel(int n_frames, int H, int W, const int32_t* __restrict__ frame_idx, co
           const double vn = sqrt(xi[3] * xi[3] + xi[4] * xi[4] + xi[5] * xi[5]);
           sh.done = (wn < p.min_step_rad && vn < gate_step_t) ? 1 : 0;
         }
+        if (trace) trace_write(p.debug, h, n_rec++, level, it, n, total, median, sh, true, xi);
       }
       __syncthreads();
       const int done = sh.done;
@@ -500,6 +544,23 @@ icp_kernel(int n_frames, int H, int W, const int32_t* __restrict__ frame_idx, co
     po[tid] = t0[tid];
   }
   if (tid == 0) { out_status[h] = GP_ICP_OK; out_residual[h] = (float)residual; out_fitness[h] = (float)fitness; }
+}
+
+// gp_debug_icp_select: out[0] = m, the entries that are not kNoPair; out[1] = radix_select's element of rank `rank`
+// among them (kNoPair when rank >= m)
+__global__ void __launch_bounds__(kThreads, 1)
+select_kernel(const unsigned* __restrict__ bits, int n, int rank, unsigned* __restrict__ out) {
+  __shared__ SelectShared sel;
+  __shared__ int count;
+  if (threadIdx.x == 0) count = 0;
+  __syncthreads();
+  int c = 0;
+  for (int i = threadIdx.x; i < n; i += kThreads) c += bits[i] != kNoPair;
+  atomicAdd(&count, c);
+  __syncthreads();
+  const int m = count;
+  const unsigned v = rank < m ? radix_select(bits, n, rank, sel) : kNoPair;
+  if (threadIdx.x == 0) { out[0] = (unsigned)m; out[1] = v; }
 }
 
 size_t align256(size_t b) { return (b + 255) & ~(size_t)255; }
@@ -566,6 +627,8 @@ extern "C" int gp_icp_refine(int n_frames, int n_hyp, int height, int width, con
   if (!frame_idx || !rendered_depth || !boxes || !T0 || !K || !out_poses || !out_status || !out_residual ||
       !out_fitness || !workspace)
     return gp_internal_fail(GP_ERR_INVALID, "null argument");
+  if (p.debug.trace && (p.debug.trace_capacity < 1 || !p.debug.trace_count))
+    return gp_internal_fail(GP_ERR_INVALID, "debug.trace needs trace_capacity >= 1 and trace_count");
   if (n_hyp == 0) return GP_OK;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const size_t plane = (size_t)height * width;
@@ -578,6 +641,17 @@ extern "C" int gp_icp_refine(int n_frames, int n_hyp, int height, int width, con
                                          p, src, dist, tgt, out_poses, out_status, out_residual, out_fitness);
   const cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return gp_internal_fail(GP_ERR_CUDA, "icp launch failed: %s", cudaGetErrorString(e));
+  gp_internal_count_launches(1);
+  return GP_OK;
+}
+
+extern "C" int gp_debug_icp_select(const uint32_t* bits, int n, int rank, uint32_t* out, void* stream) {
+  if (n < 1) return gp_internal_fail(GP_ERR_INVALID, "n %d must be >= 1", n);
+  if (rank < 0 || rank >= n) return gp_internal_fail(GP_ERR_INVALID, "rank %d outside [0, n = %d)", rank, n);
+  if (!bits || !out) return gp_internal_fail(GP_ERR_INVALID, "null argument");
+  select_kernel<<<1, kThreads, 0, static_cast<cudaStream_t>(stream)>>>(bits, n, rank, out);
+  const cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return gp_internal_fail(GP_ERR_CUDA, "icp select launch failed: %s", cudaGetErrorString(e));
   gp_internal_count_launches(1);
   return GP_OK;
 }

@@ -32,7 +32,7 @@ def make_params(debug=None, **params) -> GpIcpParams:
     p = dict(DEFAULTS, **params)
     out = GpIcpParams(**p)
     if debug:
-        out.debug = GpIcpDebug(**{k: _ptr(v) for k, v in debug.items()})
+        out.debug = GpIcpDebug(**{k: v if isinstance(v, int) else _ptr(v) for k, v in debug.items()})
     return out
 
 

@@ -300,6 +300,23 @@ int gp_render_templates(int n_views, int height, int width, int num_vertices, co
 #define GP_ICP_INVALID 4          /* frame_idx outside [0, n_frames): T0 returned */
 #define GP_ICP_LOST 5             /* an iteration found no pair, or kept fewer than 6: T0 returned */
 
+/* One ICP iteration of one hypothesis (gp_icp_debug_t.trace), 456 bytes.  Written by every iteration that associates,
+ * including the one that ends the refinement as LOST or DEGENERATE. */
+typedef struct gp_icp_trace {
+  int32_t level;                 /* L-1 .. 0 */
+  int32_t iteration;             /* 0-based within the level */
+  int32_t n;                     /* sources at this level, ceil(sources / 2^level) */
+  int32_t found;                 /* sources with a pair */
+  int32_t kept;                  /* pairs within rejection_scale x the median (0 when found = 0) */
+  int32_t done;                  /* 0 step taken, 1 step taken and the level converged, 2 degenerate, 3 lost */
+  uint32_t median_bits;          /* float bits of the median pair distance (+inf bits when found = 0) */
+  int32_t reserved;              /* 0 */
+  float Tf[12];                  /* [3,4] the fp32 correction the sources were transformed with */
+  double sums[29];               /* 21 upper-triangle entries of A^T A (row by row), 6 of A^T r, sum r^2, kept */
+  double xi[6];                  /* the solved step (omega L, v); 0 unless done is 0 or 1 */
+  double dT[12];                 /* [3,4] the fp64 correction after the step (unchanged for done 2, 3) */
+} gp_icp_trace_t;
+
 typedef struct gp_icp_debug {    /* every field nullable; test and timing hooks */
   int32_t* counts;               /* [n_hyp,2] number of targets, sources */
   int32_t* sources;              /* [n_hyp,H*W] compacted source pixel indices (row-major), first `sources` entries */
@@ -308,6 +325,9 @@ typedef struct gp_icp_debug {    /* every field nullable; test and timing hooks 
   float* pose0;                  /* [n_hyp,3,4] the correction after the centroid shift, before the first iteration */
   int32_t* iterations;           /* [n_hyp,num_levels] iterations run per level (index = level); not written for
                                     levels that were not reached */
+  gp_icp_trace_t* trace;         /* [n_hyp,trace_capacity] per-iteration records in order; needs trace_count */
+  int32_t trace_capacity;        /* >= 1 when trace is set; records past it are counted but not written */
+  int32_t* trace_count;          /* [n_hyp] records of each hypothesis (0 when it stops before iterating) */
 } gp_icp_debug_t;
 
 typedef struct gp_icp_params {
@@ -339,6 +359,11 @@ int gp_icp_refine(int n_frames, int n_hyp, int height, int width, const int32_t*
                   const float* rendered_depth, const int64_t* boxes, const float* T0, const float* K,
                   const gp_icp_params_t* params, float* out_poses, int32_t* out_status, float* out_residual,
                   float* out_fitness, void* workspace, void* stream);
+/* test hook: the exact median select of gp_icp_refine alone, in one 256-thread CTA.  bits u32 [n] (float bits of
+ * non-negative distances; 0x7f800000 = no pair, skipped) -> out u32 [2]: m = the entries that are not 0x7f800000, and
+ * the bits of the element of rank `rank` (0-based, ascending) among them, or 0x7f800000 when rank >= m.  n >= 1,
+ * 0 <= rank < n; arguments are checked before any device work. */
+int gp_debug_icp_select(const uint32_t* bits, int n, int rank, uint32_t* out, void* stream);
 
 /* --- diagnostics ----------------------------------------------------------------------------------------- */
 /* number of kernels this library has launched since load (all handles); used for bench.py's `gpu_launches` */

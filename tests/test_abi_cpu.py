@@ -175,3 +175,22 @@ def test_debug_kernel_entries_reject_bad_arguments_without_a_gpu(lib):
         assert ln(8, **{null: None}) == -1 and b"null" in lib.gp_last_error()
     for M in (0, -5):
         assert ln(M) == -1 and b"M must be" in lib.gp_last_error()
+
+
+def test_icp_debug_hooks_reject_bad_arguments_without_a_gpu(lib):
+    """gp_debug_icp_select checks n, rank and its pointers, and gp_icp_refine checks the trace fields, before either
+    touches a device; the trace record has the header's 456-byte layout."""
+    fake = 1 << 20                                   # never dereferenced: every call below fails validation first
+    sel = lambda n, rank, bits=fake, out=fake: lib.gp_debug_icp_select(bits, n, rank, out, None)
+    for n, rank, word in ((0, 0, b"n 0"), (-3, 0, b"n -3"), (5, 5, b"rank 5"), (5, -1, b"rank -1"),
+                          (1, 1, b"rank 1")):
+        assert sel(n, rank) == -1 and word in lib.gp_last_error(), (n, rank)
+    for null in ("bits", "out"):
+        assert sel(4, 0, **{null: None}) == -1 and b"null" in lib.gp_last_error()
+    assert C.sizeof(_lib.GpIcpTrace) == 456 and _lib.GpIcpTrace.sums.offset == 80
+    p = _lib.GpIcpParams(unit_per_m=1000.0, min_points=1000, num_levels=4, max_iters=100, rejection_scale=2.5,
+                         max_residual=0.01, min_step_rad=1e-6, min_step_m=1e-6)
+    for cap, count in ((0, fake), (-1, fake), (8, None)):
+        p.debug = _lib.GpIcpDebug(trace=fake, trace_capacity=cap, trace_count=count)
+        assert lib.gp_icp_refine(1, 1, 480, 640, *[fake] * 6, C.byref(p), *[fake] * 5, None) == -1, (cap, count)
+        assert b"trace" in lib.gp_last_error()
