@@ -186,3 +186,29 @@ def check(status: int) -> None:
     if status != 0:
         msg = load().gp_last_error()
         raise GigaPoseNativeError(f"gigapose_b200 error {status}: {msg.decode() if msg else '?'}")
+
+
+def ptr(t):
+    """Device address of a tensor, or None (a NULL pointer) for None."""
+    return None if t is None else t.data_ptr()
+
+
+def cuda_device(device, what: str):
+    """torch.device of a CUDA `device` with its index resolved ("cuda" = the current device); refuses anything else."""
+    import torch
+    device = torch.device(device)
+    if device.type != "cuda":
+        raise GigaPoseNativeError(f"{what} on CUDA devices only (no CPU fallback)")
+    if device.index is None:
+        device = torch.device("cuda", torch.cuda.current_device())
+    return device
+
+
+def aligned_buffer(nbytes: int, device, zero: bool = False):
+    """Caller-owned device memory for the library, which wants its bank / workspace / weight memory 1024-byte aligned
+    (the TMA swizzle atoms).  Returns (owner, view): `view` is the `nbytes`-byte slice of `owner` that starts on a
+    1024-byte boundary; keep `owner` alive as long as the library holds the address."""
+    import torch
+    owner = (torch.zeros if zero else torch.empty)(nbytes + 1024, dtype=torch.uint8, device=device)
+    off = (-owner.data_ptr()) % 1024
+    return owner, owner[off:off + nbytes]

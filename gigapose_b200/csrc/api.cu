@@ -4,147 +4,13 @@
 #include "../../include/gigapose_b200.h"
 #include "gigapose_kernels.h"
 
-#include <atomic>
 #include <dlfcn.h>
-#include <cstdarg>
-#include <cstdio>
 #include <cstdlib>
-#include <cstring>
+#include <memory>
 #include <new>
-#include <string>
 
-int gp_internal_make_map_nhwc(CUtensorMap* map, void* ptr, uint64_t C, uint64_t W, uint64_t H, uint64_t N, uint32_t out_w,
-                              uint32_t out_h, uint32_t stride);
-int gp_internal_make_map_raw(CUtensorMap* map, void* ptr, int rank, const uint64_t* dims, const uint64_t* strides_bytes,
-                             const uint32_t* box, const uint32_t* elem_strides);
-int gp_internal_make_map_ex(CUtensorMap* map, void* ptr, uint64_t rows, uint64_t cols, uint32_t box_cols, uint32_t box_rows,
-                            int swizzle_bytes);
-int gp_internal_make_map(CUtensorMap* map, void* ptr, uint64_t rows, uint64_t cols, uint32_t box_rows);
-
-namespace {
-
-thread_local std::string g_last_error;
-std::atomic<uint64_t> g_launches{0};
-
-int fail(int code, const char* fmt, ...) {
-  char buf[512];
-  va_list ap;
-  va_start(ap, fmt);
-  vsnprintf(buf, sizeof(buf), fmt, ap);
-  va_end(ap);
-  g_last_error = buf;
-  return code;
-}
-
-#define GP_CUDA(expr)                                                                                     \
-  do {                                                                                                    \
-    cudaError_t _e = (expr);                                                                              \
-    if (_e != cudaSuccess) return fail(GP_ERR_CUDA, "%s failed: %s", #expr, cudaGetErrorString(_e));     \
-  } while (0)
-
-constexpr size_t kAlign = 1024;
-inline size_t align_up(size_t x) { return (x + kAlign - 1) / kAlign * kAlign; }
-
-// bump allocator over caller memory; with base == nullptr it only measures
-struct Carver {
-  uint8_t* base;
-  size_t off = 0;
-  explicit Carver(void* b) : base(static_cast<uint8_t*>(b)) {}
-  template <typename T>
-  T* take(size_t count) {
-    T* p = base ? reinterpret_cast<T*>(base + off) : nullptr;
-    off += align_up(count * sizeof(T));
-    return p;
-  }
-};
-
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                  const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                                  CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-EncodeTiledFn get_encode_fn() {
-  static EncodeTiledFn fn = nullptr;
-  if (!fn) {
-    void* p = nullptr;
-    cudaDriverEntryPointQueryResult q;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) == cudaSuccess &&
-        q == cudaDriverEntryPointSuccess)
-      fn = reinterpret_cast<EncodeTiledFn>(p);
-  }
-  return fn;
-}
-
-}  // namespace
-
-int gp_internal_fail(int code, const char* fmt, ...) {
-  char buf[512];
-  va_list ap;
-  va_start(ap, fmt);
-  vsnprintf(buf, sizeof(buf), fmt, ap);
-  va_end(ap);
-  g_last_error = buf;
-  return code;
-}
-void gp_internal_count_launches(int n) { g_launches += n; }
-namespace gp {
-// Off by default: the 1-CTA-per-SM kernels hold most of the shared memory until they exit, so a dependent grid cannot
-// become resident early enough to hide much more than its own prologue (not measured on H100; scripts/pdl_ab.py does).
-// GIGAPOSE_PDL=1 turns it on (read at every launch).
-bool pdl_enabled() {
-  const char* ev = getenv("GIGAPOSE_PDL");
-  return ev ? (ev[0] != '0') : false;
-}
-}  // namespace gp
-
-// generic 2-D bf16 plane map [rows, cols] (cols contiguous) with explicit box and swizzle (64 or 128 = box_cols * 2 bytes)
-int gp_internal_make_map_ex(CUtensorMap* map, void* ptr, uint64_t rows, uint64_t cols, uint32_t box_cols, uint32_t box_rows,
-                            int swizzle_bytes) {
-  EncodeTiledFn enc = get_encode_fn();
-  if (!enc) return fail(GP_ERR_UNSUPPORTED, "cuTensorMapEncodeTiled not available from this driver");
-  cuuint64_t dims[2] = {cols, rows};
-  cuuint64_t strides[1] = {cols * sizeof(uint16_t)};
-  cuuint32_t box[2] = {box_cols, box_rows};
-  cuuint32_t estr[2] = {1, 1};
-  const CUtensorMapSwizzle sw = swizzle_bytes == 128 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B;
-  CUresult r = enc(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, ptr, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, sw,
-                   CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) return fail(GP_ERR_CUDA, "cuTensorMapEncodeTiled failed with CUresult %d", (int)r);
-  return GP_OK;
-}
-// NHWC bf16 plane [N, H, W, C] as a 4-D tensor {C, W, H, N}; box = 32 channels x out_w x out_h output positions taken
-// with element stride `stride` along x and y (the traversal box spans out * stride input elements).  Coordinates that
-// fall outside [0,W) x [0,H) -- the zero padding of a convolution -- are filled with zeros by TMA.
-int gp_internal_make_map_nhwc(CUtensorMap* map, void* ptr, uint64_t C, uint64_t W, uint64_t H, uint64_t N, uint32_t out_w,
-                              uint32_t out_h, uint32_t stride) {
-  EncodeTiledFn enc = get_encode_fn();
-  if (!enc) return fail(GP_ERR_UNSUPPORTED, "cuTensorMapEncodeTiled not available from this driver");
-  cuuint64_t dims[4] = {C, W, H, N};
-  cuuint64_t strides[3] = {C * sizeof(uint16_t), W * C * sizeof(uint16_t), H * W * C * sizeof(uint16_t)};
-  cuuint32_t box[4] = {32, out_w * stride, out_h * stride, 1};
-  cuuint32_t estr[4] = {1, stride, stride, 1};
-  CUresult r = enc(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, ptr, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                   CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) return fail(GP_ERR_CUDA, "cuTensorMapEncodeTiled (NHWC) failed with CUresult %d", (int)r);
-  return GP_OK;
-}
-// bf16 tensor map with caller-chosen dimensions / byte strides (rank <= 5, SWIZZLE_64B): used for views whose rows
-// overlap in memory (the stem's sliding 8-pixel windows, ist_trunk.cu)
-int gp_internal_make_map_raw(CUtensorMap* map, void* ptr, int rank, const uint64_t* dims, const uint64_t* strides_bytes,
-                             const uint32_t* box, const uint32_t* elem_strides) {
-  EncodeTiledFn enc = get_encode_fn();
-  if (!enc) return fail(GP_ERR_UNSUPPORTED, "cuTensorMapEncodeTiled not available from this driver");
-  cuuint64_t d[5], st[4];
-  cuuint32_t b[5], es[5];
-  for (int i = 0; i < rank; ++i) { d[i] = dims[i]; b[i] = box[i]; es[i] = elem_strides[i]; if (i + 1 < rank) st[i] = strides_bytes[i]; }
-  CUresult r = enc(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, rank, ptr, d, st, b, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                   CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) return fail(GP_ERR_CUDA, "cuTensorMapEncodeTiled (raw, rank %d) failed with CUresult %d", rank, (int)r);
-  return GP_OK;
-}
-// [rows, cols] plane, box = 32 columns (SWIZZLE_64B) x box_rows
-int gp_internal_make_map(CUtensorMap* map, void* ptr, uint64_t rows, uint64_t cols, uint32_t box_rows) {
-  return gp_internal_make_map_ex(map, ptr, rows, cols, 32, box_rows, 64);
-}
+using gp::Carver;
+using gp::fail;
 
 namespace {
 
@@ -152,7 +18,7 @@ namespace {
 // 64-byte rows [images * 32 * 256, 32]; box = 32 channels (64 B, SWIZZLE_64B) x box_rows patches of one k-block slab
 // (256 = all patches of a template, 128 = one t-half of a query)
 int make_plane_map(CUtensorMap* map, void* ptr, uint64_t images, uint32_t box_rows) {
-  return gp_internal_make_map_ex(map, ptr, images * 32ull * GP_NUM_PATCHES, 32, 32, box_rows, 64);
+  return gp::make_map_ex(map, ptr, images * 32ull * GP_NUM_PATCHES, 32, 32, box_rows, 64);
 }
 
 struct Bank {
@@ -295,9 +161,7 @@ int resolve_nccl() {
 
 extern "C" {
 
-const char* gp_last_error(void) { return g_last_error.c_str(); }
 int gp_abi_version(void) { return GP_ABI_VERSION; }
-uint64_t gp_launch_count(void) { return g_launches.load(); }
 
 int gp_query_sizes(const gp_config_t* cfg, size_t* bank_bytes, size_t* workspace_bytes) {
   if (int e = validate(cfg)) return e;
@@ -312,21 +176,18 @@ int gp_query_sizes(const gp_config_t* cfg, size_t* bank_bytes, size_t* workspace
 int gp_create(const gp_config_t* cfg, void* bank_mem, void* workspace_mem, gp_handle_t* out) {
   if (int e = validate(cfg)) return e;
   if (!bank_mem || !workspace_mem || !out) return fail(GP_ERR_INVALID, "null pointer argument");
-  if (((uintptr_t)bank_mem | (uintptr_t)workspace_mem) & (kAlign - 1))
-    return fail(GP_ERR_INVALID, "bank and workspace must be %zu-byte aligned", kAlign);
-  GP_CUDA(cudaSetDevice(cfg->device));
-  cudaDeviceProp prop;
-  GP_CUDA(cudaGetDeviceProperties(&prop, cfg->device));
-  if (prop.major != 9 || prop.minor != 0)
-    return fail(GP_ERR_UNSUPPORTED, "device %d is sm_%d%d; this library contains sm_90a code only", cfg->device,
-                prop.major, prop.minor);
-  if ((int)prop.sharedMemPerBlockOptin < gp::sim_search_smem_bytes())
-    return fail(GP_ERR_UNSUPPORTED, "device offers %zu B of shared memory per block, kernel needs %d",
-                prop.sharedMemPerBlockOptin, gp::sim_search_smem_bytes());
-  gp_context* h = new (std::nothrow) gp_context();
+  if (((uintptr_t)bank_mem | (uintptr_t)workspace_mem) & (gp::kAlign - 1))
+    return fail(GP_ERR_INVALID, "bank and workspace must be %zu-byte aligned", gp::kAlign);
+  int num_sms = 0, smem_optin = 0;
+  if (int e = gp::open_device(cfg->device, &num_sms)) return e;
+  GP_CUDA(cudaDeviceGetAttribute(&smem_optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, cfg->device));
+  if (smem_optin < gp::sim_search_smem_bytes())
+    return fail(GP_ERR_UNSUPPORTED, "device offers %d B of shared memory per block, kernel needs %d", smem_optin,
+                gp::sim_search_smem_bytes());
+  std::unique_ptr<gp_context> h(new (std::nothrow) gp_context());
   if (!h) return fail(GP_ERR_INVALID, "out of host memory");
   h->cfg = *cfg;
-  h->num_sms = prop.multiProcessorCount;
+  h->num_sms = num_sms;
   h->mlp_set = false;
   h->cur_B = 0;
   {
@@ -343,32 +204,24 @@ int gp_create(const gp_config_t* cfg, void* bank_mem, void* workspace_mem, gp_ha
   carve_workspace(cw, *cfg, &h->ws);
   const uint64_t bank_rows = (uint64_t)cfg->num_objects * cfg->num_templates;   // images
   const uint64_t q_rows = (uint64_t)cfg->max_batch;
+  const uint64_t rows = (uint64_t)cfg->max_batch * cfg->top_k * GP_NUM_PATCHES;
+  uint16_t* h1_hi = reinterpret_cast<uint16_t*>(h->ws.hidden1);
+  uint16_t* h1_lo = h1_hi + rows * 1024;
+  const uint64_t dims[2] = {512, rows}, strides[1] = {1024 * sizeof(uint16_t)};
+  const uint32_t box[2] = {32, 128}, estr[2] = {1, 1};
   int e;
   if ((e = make_plane_map(&h->tm_t_hi, h->bank.hi, bank_rows, 256)) || (e = make_plane_map(&h->tm_t_lo, h->bank.lo, bank_rows, 256)) ||
-      (e = make_plane_map(&h->tm_q_hi, h->ws.q_hi, q_rows, 128)) || (e = make_plane_map(&h->tm_q_lo, h->ws.q_lo, q_rows, 128))) {
-    delete h;
+      (e = make_plane_map(&h->tm_q_hi, h->ws.q_hi, q_rows, 128)) || (e = make_plane_map(&h->tm_q_lo, h->ws.q_lo, q_rows, 128)) ||
+      (e = gp::make_map(&h->tm_ma_hi, h->ws.mlp_a_hi, rows, 512, 128)) || (e = gp::make_map(&h->tm_ma_lo, h->ws.mlp_a_lo, rows, 512, 128)) ||
+      (e = gp::make_map_raw(&h->tm_h1s_hi, h1_hi, 2, dims, strides, box, estr)) ||
+      (e = gp::make_map_raw(&h->tm_h1s_lo, h1_lo, 2, dims, strides, box, estr)) ||
+      (e = gp::make_map_raw(&h->tm_h1i_hi, h1_hi + 512, 2, dims, strides, box, estr)) ||
+      (e = gp::make_map_raw(&h->tm_h1i_lo, h1_lo + 512, 2, dims, strides, box, estr)) ||
+      (e = gp::make_map(&h->tm_w1_hi, h->ws.w1_hi, 1024, 512, 256)) || (e = gp::make_map(&h->tm_w1_lo, h->ws.w1_lo, 1024, 512, 256)) ||
+      (e = gp::make_map(&h->tm_w2s_hi, h->ws.w2s_hi, 256, 512, 256)) || (e = gp::make_map(&h->tm_w2s_lo, h->ws.w2s_lo, 256, 512, 256)) ||
+      (e = gp::make_map(&h->tm_w2i_hi, h->ws.w2i_hi, 256, 512, 256)) || (e = gp::make_map(&h->tm_w2i_lo, h->ws.w2i_lo, 256, 512, 256)))
     return e;
-  }
-  {
-    const uint64_t rows = (uint64_t)cfg->max_batch * cfg->top_k * GP_NUM_PATCHES;
-    uint16_t* h1_hi = reinterpret_cast<uint16_t*>(h->ws.hidden1);
-    uint16_t* h1_lo = h1_hi + rows * 1024;
-    const uint64_t dims[2] = {512, rows}, strides[1] = {1024 * sizeof(uint16_t)};
-    const uint32_t box[2] = {32, 128}, estr[2] = {1, 1};
-    int e;
-    if ((e = gp_internal_make_map(&h->tm_ma_hi, h->ws.mlp_a_hi, rows, 512, 128)) || (e = gp_internal_make_map(&h->tm_ma_lo, h->ws.mlp_a_lo, rows, 512, 128)) ||
-        (e = gp_internal_make_map_raw(&h->tm_h1s_hi, h1_hi, 2, dims, strides, box, estr)) ||
-        (e = gp_internal_make_map_raw(&h->tm_h1s_lo, h1_lo, 2, dims, strides, box, estr)) ||
-        (e = gp_internal_make_map_raw(&h->tm_h1i_hi, h1_hi + 512, 2, dims, strides, box, estr)) ||
-        (e = gp_internal_make_map_raw(&h->tm_h1i_lo, h1_lo + 512, 2, dims, strides, box, estr)) ||
-        (e = gp_internal_make_map(&h->tm_w1_hi, h->ws.w1_hi, 1024, 512, 256)) || (e = gp_internal_make_map(&h->tm_w1_lo, h->ws.w1_lo, 1024, 512, 256)) ||
-        (e = gp_internal_make_map(&h->tm_w2s_hi, h->ws.w2s_hi, 256, 512, 256)) || (e = gp_internal_make_map(&h->tm_w2s_lo, h->ws.w2s_lo, 256, 512, 256)) ||
-        (e = gp_internal_make_map(&h->tm_w2i_hi, h->ws.w2i_hi, 256, 512, 256)) || (e = gp_internal_make_map(&h->tm_w2i_lo, h->ws.w2i_lo, 256, 512, 256))) {
-      delete h;
-      return e;
-    }
-  }
-  *out = h;
+  *out = h.release();
   return GP_OK;
 }
 
@@ -403,7 +256,6 @@ int gp_normalize_patch_tokens(int b, const float* x_prenorm, float* out, void* s
   GP_CUDA(gp::launch_split_descriptors(x_prenorm + GP_AE_DIM, (long long)b * GP_NUM_PATCHES, GP_AE_DIM, GP_NUM_PATCHES,
                                        (long long)(GP_NUM_PATCHES + 1) * GP_AE_DIM, GP_AE_DIM, 1, 1, 0, nullptr, nullptr, out,
                                        static_cast<cudaStream_t>(stream)));
-  g_launches += 1;
   return GP_OK;
 }
 
@@ -422,11 +274,9 @@ int gp_bank_write(gp_handle_t h, int obj, int tmpl0, int n, const float* feat, i
   const size_t plane_off = slot * GP_NUM_PATCHES * GP_AE_DIM;
   if (int e = split_features(feat, feat_layout, n, norm_passes, h->bank.hi + plane_off, h->bank.lo + plane_off, s)) return e;
   GP_CUDA(gp::launch_sample_mask16(mask, n, H, W, h->bank.mask16 + slot * GP_NUM_PATCHES, s));
-  g_launches += 2;
   if (ist_feat) {
     if (c.ist_bank_global) return fail(GP_ERR_INVALID, "cfg.ist_bank_global = 1: write IST features with gp_bank_write_ist (global ids)");
     GP_CUDA(gp::launch_transpose_cp(ist_feat, n, GP_IST_DIM, h->bank.ist + slot * GP_NUM_PATCHES * GP_IST_DIM, s));
-    g_launches += 1;
   }
   return GP_OK;
 }
@@ -442,7 +292,6 @@ int gp_bank_write_ist(gp_handle_t h, int obj, int tmpl0, int n, const float* ist
   float* dst = h->bank.ist + ((size_t)obj * Ti + tmpl0) * GP_NUM_PATCHES * GP_IST_DIM;
   if (ist_layout == GP_LAYOUT_CHANNEL_MAJOR) {
     GP_CUDA(gp::launch_transpose_cp(ist_feat, n, GP_IST_DIM, dst, s));
-    g_launches += 1;
   } else if (ist_layout == GP_LAYOUT_PATCH_MAJOR) {
     GP_CUDA(cudaMemcpyAsync(dst, ist_feat, (size_t)n * GP_NUM_PATCHES * GP_IST_DIM * sizeof(float), cudaMemcpyDeviceToDevice, s));
   } else {
@@ -483,7 +332,6 @@ int gp_set_ist_weights(gp_handle_t h, const float* const w[12], int use_tanh, vo
   GP_CUDA(gp::launch_split_planes(w[8], 256, 512, 512, ws.w2i_hi, ws.w2i_lo, s, true, kMlpWeightScale));
   GP_CUDA(cudaMemcpyAsync(ws.bias1, w[1], 512 * sizeof(float), cudaMemcpyDeviceToDevice, s));
   GP_CUDA(cudaMemcpyAsync(ws.bias1 + 512, w[7], 512 * sizeof(float), cudaMemcpyDeviceToDevice, s));
-  g_launches += 4;
   h->mlp_set = true;
   return GP_OK;
 }
@@ -500,7 +348,6 @@ int gp_set_queries(gp_handle_t h, int B, const float* q_feat, int feat_layout, i
   // object ids are clamped into [0, O) on the way in: an out-of-range label must not turn into an out-of-bounds bank
   // address (the host-side callers validate and raise; see GigaPose.retrieve)
   GP_CUDA(gp::launch_object_order(q_obj, B, h->cfg.num_objects, h->ws.q_obj, h->ws.perm, s));
-  g_launches += 3;
   h->cur_B = B;
   return GP_OK;
 }
@@ -523,7 +370,6 @@ static int run_sim(gp_context* h, int B, cudaStream_t s, float* debug_tile = nul
   p.rec_valid = h->ws.rec_valid;
   p.debug_tile = debug_tile;
   GP_CUDA(gp::launch_sim_search(h->tm_q_hi, h->tm_q_lo, h->tm_t_hi, h->tm_t_lo, p, h->num_sms, s));
-  g_launches += 1;
   return GP_OK;
 }
 
@@ -539,7 +385,6 @@ int gp_sim_candidates(gp_handle_t h, int B, const gp_candidates_t* out, void* st
   t.cand_score = out->score; t.cand_id = out->id; t.cand_pts_score = out->pts_score; t.cand_idx = out->idx;
   t.cand_valid = out->valid;
   GP_CUDA(gp::launch_topk_select(t, s));
-  g_launches += 1;
   return GP_OK;
 }
 
@@ -555,7 +400,6 @@ int gp_topk_merge(gp_handle_t h, int B, int G, const gp_candidates_t* g, size_t 
   m.id_src = reinterpret_cast<long long*>(out->id_src); m.score_src = out->score_src; m.score_pts = out->score_pts;
   m.tar_pts = reinterpret_cast<long long*>(out->tar_pts); m.src_pts = reinterpret_cast<long long*>(out->src_pts);
   GP_CUDA(gp::launch_topk_merge_expand(m, static_cast<cudaStream_t>(stream)));
-  g_launches += 1;
   return GP_OK;
 }
 
@@ -579,7 +423,6 @@ int gp_ist_mlp(gp_handle_t h, int b0, int n, const float* q_ist, int ist_layout,
   if (ist_layout == GP_LAYOUT_CHANNEL_MAJOR) {
     GP_CUDA(gp::launch_transpose_cp(q_ist, n, GP_IST_DIM, h->ws.q_ist, s));
     q_pm = h->ws.q_ist;
-    g_launches += 1;
   } else if (ist_layout != GP_LAYOUT_PATCH_MAJOR) {
     return fail(GP_ERR_INVALID, "unknown IST feature layout %d", ist_layout);
   }
@@ -596,7 +439,6 @@ int gp_ist_mlp(gp_handle_t h, int b0, int n, const float* q_ist, int ist_layout,
   p.row_count = h->ws.row_count; p.row_ids = h->ws.row_ids; p.hidden1 = h->ws.hidden1; p.hidden2 = h->ws.hidden2;
   if (!h->mlp_tc) {
     GP_CUDA(gp::launch_ist_mlp(h->mlp, p, s));
-    g_launches += 4;
     return GP_OK;
   }
   // tensor-core form: compacted valid rows (device-side count, no host sync) -> 512 -> [512 | 512] -> 256 + 256 -> heads.
@@ -621,7 +463,6 @@ int gp_ist_mlp(gp_handle_t h, int b0, int n, const float* q_ist, int ist_layout,
   g.bias = h->mlp.i_b2; g.x = h2i;
   GP_CUDA(gp::launch_vit_gemm(h->tm_h1i_hi, h->tm_h1i_lo, h->tm_w2i_hi, h->tm_w2i_lo, g, h->num_sms, s));
   GP_CUDA(gp::launch_mlp_head_rows(h->mlp, p, h2s, h2i, s));
-  g_launches += 6;
   return GP_OK;
 }
 
@@ -642,7 +483,6 @@ int gp_ransac(int n, float pixel_threshold, int patch_size, const int64_t* src_p
   p.in_score = reinterpret_cast<long long*>(out->inlier_scores);
   p.in_count = out->inlier_count;
   GP_CUDA(gp::launch_ransac(p, static_cast<cudaStream_t>(stream)));
-  g_launches += 1;
   return GP_OK;
 }
 
@@ -654,7 +494,6 @@ int gp_pose_recover(int B, int k, int num_templates, const int32_t* q_obj, const
   if (B < 1 || k < 1 || num_templates < 1) return fail(GP_ERR_INVALID, "B, k and num_templates must be >= 1");
   GP_CUDA(gp::launch_pose_only(B * k, k, num_templates, q_obj, q_K, q_M, reinterpret_cast<const long long*>(id_src), M,
                                tmpl_K, tmpl_M, tmpl_pose, poses, static_cast<cudaStream_t>(stream)));
-  g_launches += 1;
   return GP_OK;
 }
 
@@ -687,7 +526,6 @@ int gp_sort_and_pose(gp_handle_t h, int b0, int n, int sort_by_inliers, const fl
   p.o_in_score = reinterpret_cast<long long*>(o->ransac.inlier_scores);
   p.o_scores = o->scores; p.o_poses = o->poses;
   GP_CUDA(gp::launch_sort_and_pose(p, static_cast<cudaStream_t>(stream)));
-  g_launches += 1;
   return GP_OK;
 }
 
@@ -733,21 +571,7 @@ int gp_time_sim_kernel(gp_handle_t h, int B, int iters, float* avg_ms, void* str
   if (!h || !avg_ms || iters < 1) return fail(GP_ERR_INVALID, "bad argument");
   if (B != h->cur_B) return fail(GP_ERR_STATE, "gp_set_queries staged %d queries, timing asked for %d", h->cur_B, B);
   cudaStream_t s = static_cast<cudaStream_t>(stream);
-  cudaEvent_t e0, e1;
-  GP_CUDA(cudaEventCreate(&e0));
-  GP_CUDA(cudaEventCreate(&e1));
-  if (int e = run_sim(h, B, s)) return e;   // warm-up
-  GP_CUDA(cudaEventRecord(e0, s));
-  for (int i = 0; i < iters; ++i)
-    if (int e = run_sim(h, B, s)) return e;
-  GP_CUDA(cudaEventRecord(e1, s));
-  GP_CUDA(cudaEventSynchronize(e1));
-  float ms = 0.f;
-  GP_CUDA(cudaEventElapsedTime(&ms, e0, e1));
-  cudaEventDestroy(e0);
-  cudaEventDestroy(e1);
-  *avg_ms = ms / iters;
-  return GP_OK;
+  return gp::time_runs(s, iters, avg_ms, [&] { return run_sim(h, B, s); });
 }
 
 }  // extern "C"

@@ -50,8 +50,7 @@
 #include "../../include/gigapose_b200.h"
 #include "gigapose_kernels.h"
 
-extern int gp_internal_fail(int code, const char* fmt, ...);
-extern void gp_internal_count_launches(int n);
+using gp::fail;
 
 namespace {
 
@@ -568,10 +567,10 @@ size_t align256(size_t b) { return (b + 255) & ~(size_t)255; }
 size_t scene_bytes(int n_frames, int H, int W) { return align256((size_t)n_frames * H * W * 9 * sizeof(float)); }
 
 int check_sizes(int n_frames, int n_hyp, int H, int W) {
-  if (n_frames < 1 || n_frames > 65535) return gp_internal_fail(GP_ERR_INVALID, "n_frames %d outside [1, 65535]", n_frames);
-  if (n_hyp < 0 || n_hyp > 65535) return gp_internal_fail(GP_ERR_INVALID, "n_hyp %d outside [0, 65535]", n_hyp);
+  if (n_frames < 1 || n_frames > 65535) return fail(GP_ERR_INVALID, "n_frames %d outside [1, 65535]", n_frames);
+  if (n_hyp < 0 || n_hyp > 65535) return fail(GP_ERR_INVALID, "n_hyp %d outside [0, 65535]", n_hyp);
   if (H < kMinSide || W < kMinSide || H > kMaxSide || W > kMaxSide)
-    return gp_internal_fail(GP_ERR_INVALID, "image size %d x %d outside [%d, %d]", H, W, kMinSide, kMaxSide);
+    return fail(GP_ERR_INVALID, "image size %d x %d outside [%d, %d]", H, W, kMinSide, kMaxSide);
   return GP_OK;
 }
 
@@ -579,7 +578,7 @@ int check_sizes(int n_frames, int n_hyp, int H, int W) {
 
 extern "C" int gp_icp_query_sizes(int n_frames, int n_hyp, int height, int width, size_t* workspace_bytes) {
   if (const int rc = check_sizes(n_frames, n_hyp, height, width)) return rc;
-  if (!workspace_bytes) return gp_internal_fail(GP_ERR_INVALID, "null workspace_bytes");
+  if (!workspace_bytes) return fail(GP_ERR_INVALID, "null workspace_bytes");
   *workspace_bytes = scene_bytes(n_frames, height, width) + (size_t)n_hyp * height * width * 3 * sizeof(int);
   return GP_OK;
 }
@@ -587,9 +586,9 @@ extern "C" int gp_icp_query_sizes(int n_frames, int n_hyp, int height, int width
 extern "C" int gp_icp_prepare_scene(int n_frames, int height, int width, const float* depth, const float* K,
                                     float unit_per_m, void* workspace, void* stream) {
   if (const int rc = check_sizes(n_frames, 0, height, width)) return rc;
-  if (!depth || !K || !workspace) return gp_internal_fail(GP_ERR_INVALID, "null argument");
+  if (!depth || !K || !workspace) return fail(GP_ERR_INVALID, "null argument");
   if (!(unit_per_m > 0.f) || !isfinite(unit_per_m))
-    return gp_internal_fail(GP_ERR_INVALID, "unit_per_m must be positive and finite");
+    return fail(GP_ERR_INVALID, "unit_per_m must be positive and finite");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const size_t plane = (size_t)n_frames * height * width;
   float* map = static_cast<float*>(workspace);
@@ -597,13 +596,10 @@ extern "C" int gp_icp_prepare_scene(int n_frames, int height, int width, const f
   float* den = num + plane;
   float* S = den + plane;
   const dim3 grid((height * width + kScene - 1) / kScene, n_frames);
-  smooth_v_kernel<<<grid, kScene, 0, st>>>(height, width, depth, num, den);
-  smooth_u_kernel<<<grid, kScene, 0, st>>>(height, width, num, den, S);
-  normals_kernel<<<grid, kScene, 0, st>>>(height, width, depth, K, 0.2f * unit_per_m,
-                                          5.f * unit_per_m, S, map);
-  const cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) return gp_internal_fail(GP_ERR_CUDA, "icp scene launch failed: %s", cudaGetErrorString(e));
-  gp_internal_count_launches(3);
+  GP_CUDA(gp::launch_ex(smooth_v_kernel, grid, kScene, 0, st, 1, false, height, width, depth, num, den));
+  GP_CUDA(gp::launch_ex(smooth_u_kernel, grid, kScene, 0, st, 1, false, height, width, num, den, S));
+  GP_CUDA(gp::launch_ex(normals_kernel, grid, kScene, 0, st, 1, false, height, width, depth, K, 0.2f * unit_per_m,
+                        5.f * unit_per_m, S, map));
   return GP_OK;
 }
 
@@ -612,23 +608,23 @@ extern "C" int gp_icp_refine(int n_frames, int n_hyp, int height, int width, con
                              const float* K, const gp_icp_params_t* params, float* out_poses, int32_t* out_status,
                              float* out_residual, float* out_fitness, void* workspace, void* stream) {
   if (const int rc = check_sizes(n_frames, n_hyp, height, width)) return rc;
-  if (!params) return gp_internal_fail(GP_ERR_INVALID, "null params");
+  if (!params) return fail(GP_ERR_INVALID, "null params");
   const gp_icp_params_t& p = *params;
   if (!(p.unit_per_m > 0.f) || !isfinite(p.unit_per_m))
-    return gp_internal_fail(GP_ERR_INVALID, "unit_per_m must be positive and finite");
-  if (p.min_points < 1) return gp_internal_fail(GP_ERR_INVALID, "min_points %d must be >= 1", p.min_points);
+    return fail(GP_ERR_INVALID, "unit_per_m must be positive and finite");
+  if (p.min_points < 1) return fail(GP_ERR_INVALID, "min_points %d must be >= 1", p.min_points);
   if (p.num_levels < 1 || p.num_levels > kMaxLevels)
-    return gp_internal_fail(GP_ERR_INVALID, "num_levels %d outside [1, %d]", p.num_levels, kMaxLevels);
-  if (p.max_iters < 1 || p.max_iters > 100000) return gp_internal_fail(GP_ERR_INVALID, "max_iters %d outside [1, 100000]", p.max_iters);
+    return fail(GP_ERR_INVALID, "num_levels %d outside [1, %d]", p.num_levels, kMaxLevels);
+  if (p.max_iters < 1 || p.max_iters > 100000) return fail(GP_ERR_INVALID, "max_iters %d outside [1, 100000]", p.max_iters);
   if (!(p.rejection_scale > 0.f) || !isfinite(p.rejection_scale))
-    return gp_internal_fail(GP_ERR_INVALID, "rejection_scale must be positive and finite");
+    return fail(GP_ERR_INVALID, "rejection_scale must be positive and finite");
   if (!(p.max_residual >= 0.f) || !(p.min_step_rad >= 0.f) || !(p.min_step_m >= 0.f))
-    return gp_internal_fail(GP_ERR_INVALID, "max_residual, min_step_rad and min_step_m must be >= 0");
+    return fail(GP_ERR_INVALID, "max_residual, min_step_rad and min_step_m must be >= 0");
   if (!frame_idx || !rendered_depth || !boxes || !T0 || !K || !out_poses || !out_status || !out_residual ||
       !out_fitness || !workspace)
-    return gp_internal_fail(GP_ERR_INVALID, "null argument");
+    return fail(GP_ERR_INVALID, "null argument");
   if (p.debug.trace && (p.debug.trace_capacity < 1 || !p.debug.trace_count))
-    return gp_internal_fail(GP_ERR_INVALID, "debug.trace needs trace_capacity >= 1 and trace_count");
+    return fail(GP_ERR_INVALID, "debug.trace needs trace_capacity >= 1 and trace_count");
   if (n_hyp == 0) return GP_OK;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const size_t plane = (size_t)height * width;
@@ -637,21 +633,16 @@ extern "C" int gp_icp_refine(int n_frames, int n_hyp, int height, int width, con
   int* src = reinterpret_cast<int*>(ws + scene_bytes(n_frames, height, width));
   unsigned* dist = reinterpret_cast<unsigned*>(src + n_hyp * plane);
   int* tgt = reinterpret_cast<int*>(dist + n_hyp * plane);
-  icp_kernel<<<n_hyp, kThreads, 0, st>>>(n_frames, height, width, frame_idx, masks, rendered_depth, boxes, T0, K, map,
-                                         p, src, dist, tgt, out_poses, out_status, out_residual, out_fitness);
-  const cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) return gp_internal_fail(GP_ERR_CUDA, "icp launch failed: %s", cudaGetErrorString(e));
-  gp_internal_count_launches(1);
+  GP_CUDA(gp::launch_ex(icp_kernel, n_hyp, kThreads, 0, st, 1, false, n_frames, height, width, frame_idx, masks,
+                        rendered_depth, boxes, T0, K, map, p, src, dist, tgt, out_poses, out_status, out_residual,
+                        out_fitness));
   return GP_OK;
 }
 
 extern "C" int gp_debug_icp_select(const uint32_t* bits, int n, int rank, uint32_t* out, void* stream) {
-  if (n < 1) return gp_internal_fail(GP_ERR_INVALID, "n %d must be >= 1", n);
-  if (rank < 0 || rank >= n) return gp_internal_fail(GP_ERR_INVALID, "rank %d outside [0, n = %d)", rank, n);
-  if (!bits || !out) return gp_internal_fail(GP_ERR_INVALID, "null argument");
-  select_kernel<<<1, kThreads, 0, static_cast<cudaStream_t>(stream)>>>(bits, n, rank, out);
-  const cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) return gp_internal_fail(GP_ERR_CUDA, "icp select launch failed: %s", cudaGetErrorString(e));
-  gp_internal_count_launches(1);
+  if (n < 1) return fail(GP_ERR_INVALID, "n %d must be >= 1", n);
+  if (rank < 0 || rank >= n) return fail(GP_ERR_INVALID, "rank %d outside [0, n = %d)", rank, n);
+  if (!bits || !out) return fail(GP_ERR_INVALID, "null argument");
+  GP_CUDA(gp::launch_ex(select_kernel, 1, kThreads, 0, static_cast<cudaStream_t>(stream), 1, false, bits, n, rank, out));
   return GP_OK;
 }

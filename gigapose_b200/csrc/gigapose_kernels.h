@@ -1,34 +1,8 @@
 // Internal kernel-launch interface shared by the .cu files and the C-ABI layer (api.cu).  Not installed.
 #pragma once
-#include <cuda_runtime.h>
-#include <cuda.h>
-#include <stdint.h>
+#include "runtime.h"
 
 namespace gp {
-
-// Launch helper shared by the .cu files: optional thread-block cluster and optional programmatic dependent launch
-// (GIGAPOSE_PDL=0 turns the latter off; kernels launched this way call pdl_wait() before touching earlier kernels' data).
-bool pdl_enabled();
-template <typename... KArgs, typename... Args>
-inline cudaError_t launch_ex(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t stream, int cluster_x,
-                             bool pdl, Args&&... args) {
-  cudaLaunchConfig_t cfg{};
-  cfg.gridDim = grid; cfg.blockDim = block; cfg.dynamicSmemBytes = smem; cfg.stream = stream;
-  cudaLaunchAttribute attr[2];
-  int na = 0;
-  if (cluster_x > 1) {
-    attr[na].id = cudaLaunchAttributeClusterDimension;
-    attr[na].val.clusterDim.x = cluster_x; attr[na].val.clusterDim.y = 1; attr[na].val.clusterDim.z = 1;
-    ++na;
-  }
-  if (pdl && pdl_enabled()) {
-    attr[na].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[na].val.programmaticStreamSerializationAllowed = 1;
-    ++na;
-  }
-  cfg.attrs = attr; cfg.numAttrs = na;
-  return cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...);
-}
 
 // ---------------------------------------------------------------- similarity search (sim_search.cu)
 struct SimSearchParams {

@@ -242,18 +242,17 @@ cudaError_t launch_mlp_gather_planes(const IstMlpParams& p, uint16_t* a_hi, uint
   if (total <= 0) return cudaSuccess;
   cudaError_t e = cudaMemsetAsync(p.row_count, 0, sizeof(int), stream);
   if (e != cudaSuccess) return e;
-  mlp_compact_kernel<<<(total + 255) / 256, 256, 0, stream>>>(p, total);          // row_ids, row_count, -1000 fill
-  mlp_gather_planes_kernel<<<(total + 7) / 8, 256, 0, stream>>>(p, reinterpret_cast<__half*>(a_hi),
-                                                               reinterpret_cast<__half*>(a_lo), total);
-  return cudaGetLastError();
+  // row_ids, row_count, -1000 fill
+  if ((e = launch_ex(mlp_compact_kernel, (total + 255) / 256, 256, 0, stream, 1, false, p, total)) != cudaSuccess) return e;
+  return launch_ex(mlp_gather_planes_kernel, (total + 7) / 8, 256, 0, stream, 1, false, p, reinterpret_cast<__half*>(a_hi),
+                   reinterpret_cast<__half*>(a_lo), total);
 }
 
 cudaError_t launch_mlp_head_rows(const IstMlpWeights& w, const IstMlpParams& p, const float* h2_scale, const float* h2_inplane,
                                  cudaStream_t stream) {
   const int total = p.B * p.k * kP;
   if (total <= 0) return cudaSuccess;
-  mlp_head_rows_kernel<<<(total + 7) / 8, 256, 0, stream>>>(p, w, h2_scale, h2_inplane, total);
-  return cudaGetLastError();
+  return launch_ex(mlp_head_rows_kernel, (total + 7) / 8, 256, 0, stream, 1, false, p, w, h2_scale, h2_inplane, total);
 }
 
 cudaError_t launch_ist_mlp(const IstMlpWeights& w, const IstMlpParams& p, cudaStream_t stream) {
@@ -261,16 +260,17 @@ cudaError_t launch_ist_mlp(const IstMlpWeights& w, const IstMlpParams& p, cudaSt
   if (total <= 0) return cudaSuccess;
   cudaError_t e = cudaMemsetAsync(p.row_count, 0, sizeof(int), stream);
   if (e != cudaSuccess) return e;
-  mlp_compact_kernel<<<(total + 255) / 256, 256, 0, stream>>>(p, total);
+  if ((e = launch_ex(mlp_compact_kernel, (total + 255) / 256, 256, 0, stream, 1, false, p, total)) != cudaSuccess) return e;
   const int mtiles = (total + BM - 1) / BM;
   // layer 1 (both heads side by side): [rows,512] x [1024,512]^T -> hidden1 [rows,1024]
-  mlp_gemm_kernel<true><<<dim3(mtiles, 1024 / BN, 1), 256, 0, stream>>>(p, w.s_w1, w.s_b1, w.i_w1, w.i_b1, nullptr, 0, 512,
-                                                                      p.hidden1, 1024);
+  if ((e = launch_ex(mlp_gemm_kernel<true>, dim3(mtiles, 1024 / BN, 1), 256, 0, stream, 1, false, p, w.s_w1, w.s_b1, w.i_w1,
+                     w.i_b1, nullptr, 0, 512, p.hidden1, 1024)) != cudaSuccess)
+    return e;
   // layer 2 per head: hidden1[:, h*512:+512] x [256,512]^T -> hidden2[:, h*256:+256]
-  mlp_gemm_kernel<false><<<dim3(mtiles, 256 / BN, 2), 256, 0, stream>>>(p, w.s_w2, w.s_b2, w.i_w2, w.i_b2, p.hidden1, 1024,
-                                                                       512, p.hidden2, 512);
-  mlp_head_kernel<<<(total + 7) / 8, 256, 0, stream>>>(p, w, total);
-  return cudaGetLastError();
+  if ((e = launch_ex(mlp_gemm_kernel<false>, dim3(mtiles, 256 / BN, 2), 256, 0, stream, 1, false, p, w.s_w2, w.s_b2, w.i_w2,
+                     w.i_b2, p.hidden1, 1024, 512, p.hidden2, 512)) != cudaSuccess)
+    return e;
+  return launch_ex(mlp_head_kernel, (total + 7) / 8, 256, 0, stream, 1, false, p, w, total);
 }
 
 }  // namespace gp

@@ -16,17 +16,12 @@
 #include "gigapose_kernels.h"
 
 #include <cuda_bf16.h>
-#include <cstdlib>
+#include <memory>
 #include <new>
 #include <vector>
 
-extern int gp_internal_fail(int code, const char* fmt, ...);
-extern void gp_internal_count_launches(int n);
-extern int gp_internal_make_map(CUtensorMap* map, void* ptr, uint64_t rows, uint64_t cols, uint32_t box_rows);
-extern int gp_internal_make_map_raw(CUtensorMap* map, void* ptr, int rank, const uint64_t* dims, const uint64_t* strides_bytes,
-                                    const uint32_t* box, const uint32_t* elem_strides);
-extern int gp_internal_make_map_nhwc(CUtensorMap* map, void* ptr, uint64_t C, uint64_t W, uint64_t H, uint64_t N,
-                                     uint32_t out_w, uint32_t out_h, uint32_t stride);
+using gp::Carver;
+using gp::fail;
 
 namespace {
 
@@ -34,14 +29,6 @@ constexpr int kIn = 224, kRes = 256, kStemOut = 128, kStemKPad = 224, kFeat = 25
 constexpr int kPadRows = kRes + 6, kPadCols = kRes + 8;     // resized crop with 3 zero rows above / below, 4 zero pixels left / right
 constexpr int kDims[4] = {128, 192, 256, 512};
 constexpr int kNumConvs = GP_IST_TRUNK_NUM_CONVS;
-constexpr size_t kAlign = 1024;
-inline size_t up(size_t x) { return (x + kAlign - 1) / kAlign * kAlign; }
-
-struct Carver {
-  uint8_t* base; size_t off = 0;
-  explicit Carver(void* b) : base(static_cast<uint8_t*>(b)) {}
-  template <typename T> T* take(size_t n) { T* p = base ? reinterpret_cast<T*>(base + off) : nullptr; off += up(n * sizeof(T)); return p; }
-};
 
 struct Planes { uint16_t *hi = nullptr, *lo = nullptr; };
 
@@ -87,12 +74,6 @@ std::vector<Conv> make_schedule() {
   add(kDims[3], kFeat, 1, 1, 0, h, gp::GEMM_ROWS_F32, x, -1, -1);                     // layer4_outconv   resnet.py:379
   return v;
 }
-
-#define GPI_CUDA(expr)                                                                                    \
-  do {                                                                                                    \
-    cudaError_t _e = (expr);                                                                              \
-    if (_e != cudaSuccess) return gp_internal_fail(GP_ERR_CUDA, "%s failed: %s", #expr, cudaGetErrorString(_e)); \
-  } while (0)
 
 __device__ __forceinline__ void split_store(float v, __nv_bfloat16* hi, __nv_bfloat16* lo, size_t i) {
   const __nv_bfloat16 h = __float2bfloat16_rn(v);
@@ -177,10 +158,8 @@ void carve_workspace(Carver& c, int max_crops, gp_ist_trunk_context* h) {
 // Runs the resize and the first `last` convolutions; `dump` (if set) receives the merged output planes of convolution
 // `last` (last = 0: the zero-bordered resized-crop planes).
 int run(gp_ist_trunk_context* h, int n, const float* crops, float* feat, int last, float* dump, cudaStream_t s) {
-  resize_pad_kernel<<<(n * kRes * kRes + 255) / 256, 256, 0, s>>>(crops, n, reinterpret_cast<uint2*>(h->stem.hi),
-                                                                  reinterpret_cast<uint2*>(h->stem.lo));
-  GPI_CUDA(cudaGetLastError());
-  int launched = 1;
+  GP_CUDA(gp::launch_ex(resize_pad_kernel, (n * kRes * kRes + 255) / 256, 256, 0, s, 1, false, crops, n,
+                        reinterpret_cast<uint2*>(h->stem.hi), reinterpret_cast<uint2*>(h->stem.lo)));
   for (int i = 0; i < last; ++i) {
     const Conv& c = h->convs[i];
     gp::GemmParams g{};
@@ -196,25 +175,22 @@ int run(gp_ist_trunk_context* h, int n, const float* crops, float* feat, int las
     } else if (!(c.k == 1 && c.stride == 1)) {
       g.conv = 1; g.Ho = c.hout; g.Wo = c.hout; g.stride = c.stride; g.pad = c.pad; g.kw = c.k; g.cblocks = c.cin / 32;
     }
-    if (c.swap) GPI_CUDA(gp::launch_vit_gemm(c.w_hi, c.w_lo, c.a_hi, c.a_lo, g, h->num_sms, s));   // filters take the 128-row slot
-    else GPI_CUDA(gp::launch_vit_gemm(c.a_hi, c.a_lo, c.w_hi, c.w_lo, g, h->num_sms, s));
-    ++launched;
+    if (c.swap) GP_CUDA(gp::launch_vit_gemm(c.w_hi, c.w_lo, c.a_hi, c.a_lo, g, h->num_sms, s));   // filters take the 128-row slot
+    else GP_CUDA(gp::launch_vit_gemm(c.a_hi, c.a_lo, c.w_hi, c.w_lo, g, h->num_sms, s));
   }
   if (dump) {
     const Planes* src = &h->stem;
     long long cnt = (long long)n * kPadRows * kPadCols * 4;
     if (last > 0) {
       const Conv& c = h->convs[last - 1];
-      if (c.out_buf < 0) return gp_internal_fail(GP_ERR_INVALID, "the last convolution writes `feat` directly; nothing to dump");
+      if (c.out_buf < 0) return fail(GP_ERR_INVALID, "the last convolution writes `feat` directly; nothing to dump");
       src = &h->act[c.out_buf];
       cnt = (long long)n * c.hout * c.hout * c.cout;
     }
-    merge_planes_kernel<<<(unsigned)((cnt + 255) / 256), 256, 0, s>>>(
-        reinterpret_cast<const __nv_bfloat16*>(src->hi), reinterpret_cast<const __nv_bfloat16*>(src->lo), cnt, dump);
-    GPI_CUDA(cudaGetLastError());
-    ++launched;
+    GP_CUDA(gp::launch_ex(merge_planes_kernel, (unsigned)((cnt + 255) / 256), 256, 0, s, 1, false,
+                          reinterpret_cast<const __nv_bfloat16*>(src->hi), reinterpret_cast<const __nv_bfloat16*>(src->lo),
+                          cnt, dump));
   }
-  gp_internal_count_launches(launched);
   return GP_OK;
 }
 
@@ -223,7 +199,7 @@ int run(gp_ist_trunk_context* h, int n, const float* crops, float* feat, int las
 extern "C" {
 
 int gp_ist_trunk_query_sizes(int max_crops, size_t* weight_bytes, size_t* workspace_bytes) {
-  if (max_crops < 1) return gp_internal_fail(GP_ERR_INVALID, "bad max_crops");
+  if (max_crops < 1) return fail(GP_ERR_INVALID, "bad max_crops");
   Carver cw(nullptr), cs(nullptr);
   carve_weights(cw, nullptr, make_schedule());
   carve_workspace(cs, max_crops, nullptr);
@@ -234,70 +210,63 @@ int gp_ist_trunk_query_sizes(int max_crops, size_t* weight_bytes, size_t* worksp
 
 int gp_ist_trunk_create(int device, int max_crops, int precision, const gp_conv_weights_t* w, void* weight_mem,
                         void* workspace_mem, void* stream, gp_ist_trunk_handle_t* out) {
-  if (max_crops < 1 || !w || !weight_mem || !workspace_mem || !out) return gp_internal_fail(GP_ERR_INVALID, "bad argument");
+  if (max_crops < 1 || !w || !weight_mem || !workspace_mem || !out) return fail(GP_ERR_INVALID, "bad argument");
   if (precision != GP_PRECISION_FP32_SPLIT && precision != GP_PRECISION_BF16)
-    return gp_internal_fail(GP_ERR_INVALID, "unknown precision %d", precision);
-  if (((uintptr_t)weight_mem | (uintptr_t)workspace_mem) & (kAlign - 1))
-    return gp_internal_fail(GP_ERR_INVALID, "weight and workspace memory must be 1024-byte aligned");
+    return fail(GP_ERR_INVALID, "unknown precision %d", precision);
+  if (((uintptr_t)weight_mem | (uintptr_t)workspace_mem) & (gp::kAlign - 1))
+    return fail(GP_ERR_INVALID, "weight and workspace memory must be 1024-byte aligned");
   for (int i = 0; i < kNumConvs; ++i)
-    if (!w[i].weight) return gp_internal_fail(GP_ERR_INVALID, "weight pointer %d is null", i);
-  GPI_CUDA(cudaSetDevice(device));
-  cudaDeviceProp prop;
-  GPI_CUDA(cudaGetDeviceProperties(&prop, device));
-  if (prop.major != 9 || prop.minor != 0) return gp_internal_fail(GP_ERR_UNSUPPORTED, "device %d is not sm_90", device);
-  gp_ist_trunk_context* h = new (std::nothrow) gp_ist_trunk_context();
-  if (!h) return gp_internal_fail(GP_ERR_INVALID, "out of host memory");
-  h->max_crops = max_crops; h->num_sms = prop.multiProcessorCount;
+    if (!w[i].weight) return fail(GP_ERR_INVALID, "weight pointer %d is null", i);
+  int num_sms = 0;
+  if (int e = gp::open_device(device, &num_sms)) return e;
+  std::unique_ptr<gp_ist_trunk_context> h(new (std::nothrow) gp_ist_trunk_context());
+  if (!h) return fail(GP_ERR_INVALID, "out of host memory");
+  h->max_crops = max_crops; h->num_sms = num_sms;
   h->passes = precision == GP_PRECISION_FP32_SPLIT ? 3 : 1;
   h->convs = make_schedule();
   Carver cw(weight_mem), cs(workspace_mem);
-  carve_weights(cw, h, h->convs);
-  carve_workspace(cs, max_crops, h);
+  carve_weights(cw, h.get(), h->convs);
+  carve_workspace(cs, max_crops, h.get());
   cudaStream_t s = static_cast<cudaStream_t>(stream);
-  cudaError_t ce = cudaMemsetAsync(const_cast<float*>(h->zero_bias), 0, 512 * sizeof(float), s);
+  GP_CUDA(cudaMemsetAsync(const_cast<float*>(h->zero_bias), 0, 512 * sizeof(float), s));
   // the zero border (and 4th channel) of the resized-crop planes is written once; resize_pad_kernel fills the interior
   const size_t stem_bytes = (size_t)max_crops * kPadRows * kPadCols * 4 * sizeof(uint16_t);
-  if (ce == cudaSuccess) ce = cudaMemsetAsync(h->stem.hi, 0, stem_bytes, s);
-  if (ce == cudaSuccess) ce = cudaMemsetAsync(h->stem.lo, 0, stem_bytes, s);
-  int e = GP_OK;
-  for (int i = 0; i < kNumConvs && !e && ce == cudaSuccess; ++i) {
+  GP_CUDA(cudaMemsetAsync(h->stem.hi, 0, stem_bytes, s));
+  GP_CUDA(cudaMemsetAsync(h->stem.lo, 0, stem_bytes, s));
+  for (int i = 0; i < kNumConvs; ++i) {
     Conv& c = h->convs[i];
     c.bias = w[i].bias;
     // weights arrive as [cout, ky, kx, cin] (BatchNorm folded): exactly the [N, K] operand with K = (tap, channel)
-    if (c.in_buf < 0) {
-      pack_stem_filter_kernel<<<(kStemOut * kStemKPad + 255) / 256, 256, 0, s>>>(
-          w[i].weight, reinterpret_cast<__nv_bfloat16*>(c.w.hi), reinterpret_cast<__nv_bfloat16*>(c.w.lo));
-      ce = cudaGetLastError();
-    } else {
-      ce = gp::launch_split_planes(w[i].weight, c.cout, c.K, c.Kpad, c.w.hi, c.w.lo, s);
-    }
-    if (ce != cudaSuccess) break;
+    if (c.in_buf < 0)
+      GP_CUDA(gp::launch_ex(pack_stem_filter_kernel, (kStemOut * kStemKPad + 255) / 256, 256, 0, s, 1, false, w[i].weight,
+                            reinterpret_cast<__nv_bfloat16*>(c.w.hi), reinterpret_cast<__nv_bfloat16*>(c.w.lo)));
+    else
+      GP_CUDA(gp::launch_split_planes(w[i].weight, c.cout, c.K, c.Kpad, c.w.hi, c.w.lo, s));
     // rows per TMA box: filters / pixels
     const uint32_t wbox = c.swap ? 128 : c.bn, pix_tile = c.swap ? 256 : 128;
-    if ((e = gp_internal_make_map(&c.w_hi, c.w.hi, c.cout, c.Kpad, wbox)) || (e = gp_internal_make_map(&c.w_lo, c.w.lo, c.cout, c.Kpad, wbox)))
-      break;
+    int e;
+    if ((e = gp::make_map(&c.w_hi, c.w.hi, c.cout, c.Kpad, wbox)) || (e = gp::make_map(&c.w_lo, c.w.lo, c.cout, c.Kpad, wbox)))
+      return e;
     if (c.in_buf < 0) {
       // stem: {32 elements = 8 pixels x 4 channels, 128 windows at a 16-byte pitch, 262 rows, crops}; a 256-pixel tile
       // is two output rows = every second input row starting at 2*yo + ky
       const uint64_t dims[4] = {32, (uint64_t)kStemOut, (uint64_t)kPadRows, (uint64_t)max_crops};
       const uint64_t strides[3] = {16, (uint64_t)kPadCols * 8, (uint64_t)kPadRows * kPadCols * 8};
       const uint32_t box[4] = {32, (uint32_t)kStemOut, (pix_tile / kStemOut) * 2, 1}, es[4] = {1, 1, 2, 1};
-      (e = gp_internal_make_map_raw(&c.a_hi, h->stem.hi, 4, dims, strides, box, es)) ||
-          (e = gp_internal_make_map_raw(&c.a_lo, h->stem.lo, 4, dims, strides, box, es));
+      (e = gp::make_map_raw(&c.a_hi, h->stem.hi, 4, dims, strides, box, es)) ||
+          (e = gp::make_map_raw(&c.a_lo, h->stem.lo, 4, dims, strides, box, es));
     } else if (c.k == 1 && c.stride == 1) {               // 1x1/1: the NHWC plane is already the [pixels, cin] operand
       const uint64_t rows = (uint64_t)max_crops * c.hin * c.hin;
-      (e = gp_internal_make_map(&c.a_hi, h->act[c.in_buf].hi, rows, c.cin, pix_tile)) ||
-          (e = gp_internal_make_map(&c.a_lo, h->act[c.in_buf].lo, rows, c.cin, pix_tile));
+      (e = gp::make_map(&c.a_hi, h->act[c.in_buf].hi, rows, c.cin, pix_tile)) ||
+          (e = gp::make_map(&c.a_lo, h->act[c.in_buf].lo, rows, c.cin, pix_tile));
     } else {
       const uint32_t ow = c.hout, oh = pix_tile / c.hout;
-      (e = gp_internal_make_map_nhwc(&c.a_hi, h->act[c.in_buf].hi, c.cin, c.hin, c.hin, max_crops, ow, oh, c.stride)) ||
-          (e = gp_internal_make_map_nhwc(&c.a_lo, h->act[c.in_buf].lo, c.cin, c.hin, c.hin, max_crops, ow, oh, c.stride));
+      (e = gp::make_map_nhwc(&c.a_hi, h->act[c.in_buf].hi, c.cin, c.hin, c.hin, max_crops, ow, oh, c.stride)) ||
+          (e = gp::make_map_nhwc(&c.a_lo, h->act[c.in_buf].lo, c.cin, c.hin, c.hin, max_crops, ow, oh, c.stride));
     }
+    if (e) return e;
   }
-  if (ce != cudaSuccess) { delete h; return gp_internal_fail(GP_ERR_CUDA, "weight packing failed: %s", cudaGetErrorString(ce)); }
-  if (e) { delete h; return e; }
-  gp_internal_count_launches(kNumConvs);
-  *out = h;
+  *out = h.release();
   return GP_OK;
 }
 
@@ -307,15 +276,15 @@ int gp_ist_trunk_destroy(gp_ist_trunk_handle_t h) {
 }
 
 int gp_ist_trunk_forward(gp_ist_trunk_handle_t h, int n, const float* crops, float* feat, void* stream) {
-  if (!h || !crops || !feat) return gp_internal_fail(GP_ERR_INVALID, "null argument");
-  if (n < 1 || n > h->max_crops) return gp_internal_fail(GP_ERR_INVALID, "batch %d outside [1, %d]", n, h->max_crops);
+  if (!h || !crops || !feat) return fail(GP_ERR_INVALID, "null argument");
+  if (n < 1 || n > h->max_crops) return fail(GP_ERR_INVALID, "batch %d outside [1, %d]", n, h->max_crops);
   return run(h, n, crops, feat, kNumConvs, nullptr, static_cast<cudaStream_t>(stream));
 }
 
 int gp_debug_ist_trunk(gp_ist_trunk_handle_t h, int n, const float* crops, int num_convs, float* activation, void* stream) {
-  if (!h || !crops || !activation) return gp_internal_fail(GP_ERR_INVALID, "null argument");
-  if (n < 1 || n > h->max_crops) return gp_internal_fail(GP_ERR_INVALID, "batch %d outside [1, %d]", n, h->max_crops);
-  if (num_convs < 0 || num_convs >= kNumConvs) return gp_internal_fail(GP_ERR_INVALID, "num_convs outside [0, %d)", kNumConvs);
+  if (!h || !crops || !activation) return fail(GP_ERR_INVALID, "null argument");
+  if (n < 1 || n > h->max_crops) return fail(GP_ERR_INVALID, "batch %d outside [1, %d]", n, h->max_crops);
+  if (num_convs < 0 || num_convs >= kNumConvs) return fail(GP_ERR_INVALID, "num_convs outside [0, %d)", kNumConvs);
   return run(h, n, crops, nullptr, num_convs, activation, static_cast<cudaStream_t>(stream));
 }
 

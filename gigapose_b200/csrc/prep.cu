@@ -116,8 +116,7 @@ __global__ void object_order_kernel(const int* __restrict__ q_obj, int B, int nu
 
 cudaError_t launch_object_order(const int* q_obj, int B, int num_objects, int* q_obj_out, int* perm, cudaStream_t stream) {
   if (B <= 0) return cudaSuccess;
-  object_order_kernel<<<(B + 127) / 128, 128, 0, stream>>>(q_obj, B, num_objects, q_obj_out, perm);
-  return cudaGetLastError();
+  return launch_ex(object_order_kernel, (B + 127) / 128, 128, 0, stream, 1, false, q_obj, B, num_objects, q_obj_out, perm);
 }
 
 cudaError_t launch_split_descriptors(const float* x, long long n_rows, int C, int rows_per_img, long long img_stride,
@@ -125,18 +124,15 @@ cudaError_t launch_split_descriptors(const float* x, long long n_rows, int C, in
                                      uint16_t* lo, float* normalized_out, cudaStream_t stream) {
   if (n_rows <= 0) return cudaSuccess;
   if (C > 256 * kMaxPerThread) return cudaErrorInvalidValue;
-  split_descriptors_kernel<<<(unsigned)n_rows, 256, 0, stream>>>(x, n_rows, C, rows_per_img, img_stride, row_stride,
-                                                                chan_stride, norm_passes, tiled,
-                                                                reinterpret_cast<__nv_bfloat16*>(hi),
-                                                                reinterpret_cast<__nv_bfloat16*>(lo), normalized_out);
-  return cudaGetLastError();
+  return launch_ex(split_descriptors_kernel, (unsigned)n_rows, 256, 0, stream, 1, false, x, n_rows, C, rows_per_img, img_stride,
+                   row_stride, chan_stride, norm_passes, tiled, reinterpret_cast<__nv_bfloat16*>(hi),
+                   reinterpret_cast<__nv_bfloat16*>(lo), normalized_out);
 }
 
 cudaError_t launch_sample_mask16(const float* mask, long long n, int H, int W, float* out, cudaStream_t stream) {
   if (n <= 0) return cudaSuccess;
   const long long total = n * 256;
-  sample_mask16_kernel<<<(unsigned)((total + 255) / 256), 256, 0, stream>>>(mask, n, H, W, out);
-  return cudaGetLastError();
+  return launch_ex(sample_mask16_kernel, (unsigned)((total + 255) / 256), 256, 0, stream, 1, false, mask, n, H, W, out);
 }
 
 cudaError_t launch_transpose_cp(const float* in, long long n, int C, float* out, cudaStream_t stream) {
@@ -144,9 +140,10 @@ cudaError_t launch_transpose_cp(const float* in, long long n, int C, float* out,
   for (long long i0 = 0; i0 < n; i0 += 32768) {          // gridDim.z limit
     const long long cnt = (n - i0 < 32768) ? (n - i0) : 32768;
     dim3 grid(256 / 32, (C + 31) / 32, (unsigned)cnt), block(32, 8);
-    transpose_cp_kernel<<<grid, block, 0, stream>>>(in + i0 * C * 256, C, out + i0 * C * 256);
+    cudaError_t e = launch_ex(transpose_cp_kernel, grid, block, 0, stream, 1, false, in + i0 * C * 256, C, out + i0 * C * 256);
+    if (e != cudaSuccess) return e;
   }
-  return cudaGetLastError();
+  return cudaSuccess;
 }
 
 }  // namespace gp

@@ -12,8 +12,7 @@
 #include "../../include/gigapose_b200.h"
 #include "gigapose_kernels.h"
 
-extern int gp_internal_fail(int code, const char* fmt, ...);
-extern void gp_internal_count_launches(int n);
+using gp::fail;
 
 namespace {
 
@@ -122,19 +121,16 @@ extern "C" int gp_crop_resize_pad(int n, int channels, int height, int width, in
                                   const int32_t* image_index, const int64_t* xyxy_boxes, const float* mask, float in_div,
                                   const float* post_sub, const float* post_div, float* out_images, float* out_mask,
                                   float* out_M, void* stream) {
-  if (n < 0 || channels < 1 || height < 1 || width < 1) return gp_internal_fail(GP_ERR_INVALID, "bad shape");
+  if (n < 0 || channels < 1 || height < 1 || width < 1) return fail(GP_ERR_INVALID, "bad shape");
   if (target_size < 128 || target_size > 4096)
-    return gp_internal_fail(GP_ERR_INVALID, "target_size %d outside [128, 4096] (smaller outputs take a different ATen path)", target_size);
-  if (!images || !xyxy_boxes || !out_images) return gp_internal_fail(GP_ERR_INVALID, "null argument");
-  if (out_mask && !mask) return gp_internal_fail(GP_ERR_INVALID, "out_mask needs mask");
-  if (!(in_div > 0.f)) return gp_internal_fail(GP_ERR_INVALID, "in_div must be positive");
+    return fail(GP_ERR_INVALID, "target_size %d outside [128, 4096] (smaller outputs take a different ATen path)", target_size);
+  if (!images || !xyxy_boxes || !out_images) return fail(GP_ERR_INVALID, "null argument");
+  if (out_mask && !mask) return fail(GP_ERR_INVALID, "out_mask needs mask");
+  if (!(in_div > 0.f)) return fail(GP_ERR_INVALID, "in_div must be positive");
   if (n == 0) return GP_OK;
   const dim3 grid((target_size * target_size + 255) / 256, n);
-  crop_resize_pad_kernel<<<grid, 256, 0, static_cast<cudaStream_t>(stream)>>>(
-      channels, height, width, target_size, images, image_index, reinterpret_cast<const long long*>(xyxy_boxes), mask, in_div,
-      post_sub, post_div, out_images, out_mask, out_M);
-  const cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) return gp_internal_fail(GP_ERR_CUDA, "crop_resize_pad launch failed: %s", cudaGetErrorString(e));
-  gp_internal_count_launches(1);
+  GP_CUDA(gp::launch_ex(crop_resize_pad_kernel, grid, 256, 0, static_cast<cudaStream_t>(stream), 1, false, channels, height,
+                        width, target_size, images, image_index, reinterpret_cast<const long long*>(xyxy_boxes), mask,
+                        in_div, post_sub, post_div, out_images, out_mask, out_M));
   return GP_OK;
 }

@@ -264,23 +264,21 @@ __global__ void pose_only_kernel(int n, int k, int T, const int* __restrict__ q_
 
 cudaError_t launch_ransac(const RansacParams& p, cudaStream_t stream) {
   if (p.n <= 0) return cudaSuccess;
-  ransac_kernel<<<p.n, 256, 0, stream>>>(p);
-  return cudaGetLastError();
+  return launch_ex(ransac_kernel, p.n, 256, 0, stream, 1, false, p);
 }
 
 cudaError_t launch_pose_only(int n, int k, int T, const int* q_obj, const float* q_K, const float* q_M,
                              const long long* id_src, const float* M, const float* tmpl_K, const float* tmpl_M,
                              const float* tmpl_pose, float* poses, cudaStream_t stream) {
   if (n <= 0) return cudaSuccess;
-  pose_only_kernel<<<(n + 127) / 128, 128, 0, stream>>>(n, k, T, q_obj, q_K, q_M, id_src, M, tmpl_K, tmpl_M, tmpl_pose, poses);
-  return cudaGetLastError();
+  return launch_ex(pose_only_kernel, (n + 127) / 128, 128, 0, stream, 1, false, n, k, T, q_obj, q_K, q_M, id_src, M, tmpl_K,
+                   tmpl_M, tmpl_pose, poses);
 }
 
 cudaError_t launch_sort_and_pose(const PoseParams& p, cudaStream_t stream) {
   if (p.B <= 0) return cudaSuccess;
   if (p.k > 32) return cudaErrorInvalidValue;
-  sort_and_pose_kernel<<<p.B, 256, 0, stream>>>(p);
-  return cudaGetLastError();
+  return launch_ex(sort_and_pose_kernel, p.B, 256, 0, stream, 1, false, p);
 }
 
 }  // namespace gp

@@ -32,8 +32,7 @@
 #include "../../include/gigapose_b200.h"
 #include "gigapose_kernels.h"
 
-extern int gp_internal_fail(int code, const char* fmt, ...);
-extern void gp_internal_count_launches(int n);
+using gp::fail;
 
 namespace {
 
@@ -309,9 +308,9 @@ boxes_kernel(int H, int W, const float* __restrict__ rgba, long long* __restrict
 constexpr int kMaxSide = 8192;
 
 int check_sizes(int max_views, int height, int width) {
-  if (max_views < 0 || max_views > 65535) return gp_internal_fail(GP_ERR_INVALID, "n_views %d outside [0, 65535]", max_views);
+  if (max_views < 0 || max_views > 65535) return fail(GP_ERR_INVALID, "n_views %d outside [0, 65535]", max_views);
   if (height < 1 || width < 1 || height > kMaxSide || width > kMaxSide)
-    return gp_internal_fail(GP_ERR_INVALID, "image size %d x %d outside [1, %d]", height, width, kMaxSide);
+    return fail(GP_ERR_INVALID, "image size %d x %d outside [1, %d]", height, width, kMaxSide);
   return GP_OK;
 }
 
@@ -319,7 +318,7 @@ int check_sizes(int max_views, int height, int width) {
 
 extern "C" int gp_render_query_sizes(int max_views, int height, int width, size_t* workspace_bytes) {
   if (const int rc = check_sizes(max_views, height, width)) return rc;
-  if (!workspace_bytes) return gp_internal_fail(GP_ERR_INVALID, "null workspace_bytes");
+  if (!workspace_bytes) return fail(GP_ERR_INVALID, "null workspace_bytes");
   *workspace_bytes = (size_t)max_views * height * width * 4 * sizeof(unsigned long long);
   return GP_OK;
 }
@@ -330,34 +329,27 @@ extern "C" int gp_render_templates(int n_views, int height, int width, int num_v
                                    const float* poses, const float* K, float z_near, void* workspace, float* rgba,
                                    float* depth, int64_t* boxes, void* stream) {
   if (const int rc = check_sizes(n_views, height, width)) return rc;
-  if (num_vertices < 0 || num_faces < 0) return gp_internal_fail(GP_ERR_INVALID, "negative mesh size");
-  if (!(z_near > 0.f) || !isfinite(z_near)) return gp_internal_fail(GP_ERR_INVALID, "z_near must be positive and finite");
-  if (!poses || !K || !workspace || !rgba || !boxes) return gp_internal_fail(GP_ERR_INVALID, "null argument");
+  if (num_vertices < 0 || num_faces < 0) return fail(GP_ERR_INVALID, "negative mesh size");
+  if (!(z_near > 0.f) || !isfinite(z_near)) return fail(GP_ERR_INVALID, "z_near must be positive and finite");
+  if (!poses || !K || !workspace || !rgba || !boxes) return fail(GP_ERR_INVALID, "null argument");
   if (num_faces > 0 && (!vertices || !faces || num_vertices < 1))
-    return gp_internal_fail(GP_ERR_INVALID, "null argument (mesh)");
-  if (texture && vertex_color) return gp_internal_fail(GP_ERR_INVALID, "give vertex_color or texture, not both");
+    return fail(GP_ERR_INVALID, "null argument (mesh)");
+  if (texture && vertex_color) return fail(GP_ERR_INVALID, "give vertex_color or texture, not both");
   if (texture && (!face_uv || tex_h < 1 || tex_w < 1))
-    return gp_internal_fail(GP_ERR_INVALID, "texture needs face_uv and a positive tex_h x tex_w");
-  if (face_uv && !texture) return gp_internal_fail(GP_ERR_INVALID, "face_uv without texture");
+    return fail(GP_ERR_INVALID, "texture needs face_uv and a positive tex_h x tex_w");
+  if (face_uv && !texture) return fail(GP_ERR_INVALID, "face_uv without texture");
   if (n_views == 0) return GP_OK;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   auto* keys = static_cast<unsigned long long*>(workspace);
   const size_t key_bytes = (size_t)n_views * height * width * 4 * sizeof(unsigned long long);
-  cudaError_t e = cudaMemsetAsync(keys, 0xFF, key_bytes, st);
-  if (e != cudaSuccess) return gp_internal_fail(GP_ERR_CUDA, "render key clear failed: %s", cudaGetErrorString(e));
-  int launches = 0;
-  if (num_faces > 0) {
-    raster_kernel<<<dim3((num_faces + kThreads - 1) / kThreads, n_views), kThreads, 0, st>>>(
-        height, width, num_vertices, vertices, num_faces, faces, poses, K, z_near, keys);
-    ++launches;
-  }
-  resolve_kernel<<<dim3((height * width + kThreads - 1) / kThreads, n_views), kThreads, 0, st>>>(
-      height, width, num_vertices, vertices, faces, vertex_color, face_uv, texture, tex_h, tex_w, constant_color, poses, K,
-      z_near, keys, rgba, depth);
-  boxes_kernel<<<n_views, kThreads, 0, st>>>(height, width, rgba, reinterpret_cast<long long*>(boxes));
-  launches += 2;
-  e = cudaGetLastError();
-  if (e != cudaSuccess) return gp_internal_fail(GP_ERR_CUDA, "render launch failed: %s", cudaGetErrorString(e));
-  gp_internal_count_launches(launches);
+  GP_CUDA(cudaMemsetAsync(keys, 0xFF, key_bytes, st));
+  if (num_faces > 0)
+    GP_CUDA(gp::launch_ex(raster_kernel, dim3((num_faces + kThreads - 1) / kThreads, n_views), kThreads, 0, st, 1, false,
+                          height, width, num_vertices, vertices, num_faces, faces, poses, K, z_near, keys));
+  GP_CUDA(gp::launch_ex(resolve_kernel, dim3((height * width + kThreads - 1) / kThreads, n_views), kThreads, 0, st, 1, false,
+                        height, width, num_vertices, vertices, faces, vertex_color, face_uv, texture, tex_h, tex_w,
+                        constant_color, poses, K, z_near, keys, rgba, depth));
+  GP_CUDA(gp::launch_ex(boxes_kernel, n_views, kThreads, 0, st, 1, false, height, width, rgba,
+                        reinterpret_cast<long long*>(boxes)));
   return GP_OK;
 }

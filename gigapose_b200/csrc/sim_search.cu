@@ -413,35 +413,23 @@ topk_merge_expand_kernel(TopkMergeParams p) {
 // ------------------------------------------------------------------------------------------------------------
 cudaError_t launch_sim_search(const CUtensorMap& q_hi, const CUtensorMap& q_lo, const CUtensorMap& t_hi,
                               const CUtensorMap& t_lo, const SimSearchParams& p, int num_sms, cudaStream_t stream) {
-  static bool configured = false;
-  if (!configured) {
-    cudaError_t e = cudaSuccess;
-    for (auto k : {sim_search_kernel<false, false>, sim_search_kernel<true, false>, sim_search_kernel<false, true>,
-                   sim_search_kernel<true, true>})
-      if (e == cudaSuccess) e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes);
-    if (e != cudaSuccess) return e;
-    configured = true;
-  }
   if (p.num_items <= 0) return cudaSuccess;
   const int grid = p.num_items < num_sms ? p.num_items : num_sms;
   const bool sign = !(p.sim_threshold > 0.f);         // negative values survive the threshold
   auto kernel = p.debug_tile ? (sign ? sim_search_kernel<true, true> : sim_search_kernel<true, false>)
                              : (sign ? sim_search_kernel<false, true> : sim_search_kernel<false, false>);
-  kernel<<<grid, kThreads, kSmemBytes, stream>>>(q_hi, q_lo, t_hi, t_lo, p);
-  return cudaGetLastError();
+  return launch_ex(kernel, grid, kThreads, kSmemBytes, stream, 1, false, q_hi, q_lo, t_hi, t_lo, p);
 }
 
 cudaError_t launch_topk_select(const TopkSelectParams& p, cudaStream_t stream) {
   if (p.B <= 0) return cudaSuccess;
   if (p.T > GP_MAX_NUM_TEMPLATES) return cudaErrorInvalidValue;     // s_val[T] must fit the default 48 KiB
-  topk_select_kernel<<<p.B, 256, p.T * sizeof(float), stream>>>(p);
-  return cudaGetLastError();
+  return launch_ex(topk_select_kernel, p.B, 256, p.T * sizeof(float), stream, 1, false, p);
 }
 
 cudaError_t launch_topk_merge_expand(const TopkMergeParams& p, cudaStream_t stream) {
   if (p.B <= 0) return cudaSuccess;
-  topk_merge_expand_kernel<<<p.B, 256, 0, stream>>>(p);
-  return cudaGetLastError();
+  return launch_ex(topk_merge_expand_kernel, p.B, 256, 0, stream, 1, false, p);
 }
 
 int sim_search_smem_bytes() { return kSmemBytes; }

@@ -306,13 +306,6 @@ cudaError_t read_attention_stamps(long long* host32) {
 cudaError_t launch_attention_tc(const CUtensorMap& hi128, const CUtensorMap& lo128, const CUtensorMap& hi16,
                                 const CUtensorMap& lo16, const uint16_t* qkv_hi, const uint16_t* qkv_lo, uint16_t* out_hi,
                                 uint16_t* out_lo, int b, int crop_stride, int passes, cudaStream_t s) {
-  static bool configured = false;
-  if (!configured) {
-    cudaError_t e = cudaFuncSetAttribute(attention_tc_kernel<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmem);
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(attention_tc_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmem);
-    if (e != cudaSuccess) return e;
-    configured = true;
-  }
   if (b <= 0) return cudaSuccess;
   const int items = b * kHeads;
   const dim3 grid(items);

@@ -429,14 +429,8 @@ namespace {
 template <bool kSwap, int kTileN, bool kF16, int kMode>
 cudaError_t launch_mode(const CUtensorMap& a_hi, const CUtensorMap& a_lo, const CUtensorMap& w_hi, const CUtensorMap& w_lo,
                         const GemmParams& p, int grid, cudaStream_t stream) {
-  auto kernel = vit_gemm_kernel<kSwap, kTileN, kF16, kMode>;
-  static bool configured = false;                  // one flag per instantiation
-  if (!configured) {
-    cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes);
-    if (e != cudaSuccess) return e;
-    configured = true;
-  }
-  return launch_ex(kernel, dim3(grid), dim3(kThreads), kSmemBytes, stream, 1, true, a_hi, a_lo, w_hi, w_lo, p);
+  return launch_ex(vit_gemm_kernel<kSwap, kTileN, kF16, kMode>, dim3(grid), dim3(kThreads), kSmemBytes, stream, 1, true, a_hi,
+                   a_lo, w_hi, w_lo, p);
 }
 }  // namespace
 

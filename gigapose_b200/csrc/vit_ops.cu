@@ -126,22 +126,19 @@ cudaError_t launch_split_planes(const float* x, long long rows, int K, int Kpad,
                                 bool f16, float pre_scale) {
   const long long total = rows * Kpad;
   if (total <= 0) return cudaSuccess;
-  if (f16) {
-    split_planes_f16_kernel<<<(unsigned)((total + 255) / 256), 256, 0, s>>>(x, rows, K, Kpad, pre_scale, reinterpret_cast<__half*>(hi),
-                                                                           reinterpret_cast<__half*>(lo));
-    return cudaGetLastError();
-  }
-  split_planes_kernel<<<(unsigned)((total + 255) / 256), 256, 0, s>>>(x, rows, K, Kpad, reinterpret_cast<__nv_bfloat16*>(hi),
-                                                                     reinterpret_cast<__nv_bfloat16*>(lo));
-  return cudaGetLastError();
+  const unsigned grid = (unsigned)((total + 255) / 256);
+  if (f16)
+    return launch_ex(split_planes_f16_kernel, grid, 256, 0, s, 1, false, x, rows, K, Kpad, pre_scale, reinterpret_cast<__half*>(hi),
+                     reinterpret_cast<__half*>(lo));
+  return launch_ex(split_planes_kernel, grid, 256, 0, s, 1, false, x, rows, K, Kpad, reinterpret_cast<__nv_bfloat16*>(hi),
+                   reinterpret_cast<__nv_bfloat16*>(lo));
 }
 
 cudaError_t launch_im2col(const float* img, int b, int Kpad, uint16_t* hi, uint16_t* lo, cudaStream_t s) {
   const long long total = (long long)b * 256 * Kpad;
   if (total <= 0) return cudaSuccess;
-  im2col_kernel<<<(unsigned)((total + 255) / 256), 256, 0, s>>>(img, b, Kpad, reinterpret_cast<__nv_bfloat16*>(hi),
-                                                               reinterpret_cast<__nv_bfloat16*>(lo));
-  return cudaGetLastError();
+  return launch_ex(im2col_kernel, (unsigned)((total + 255) / 256), 256, 0, s, 1, false, img, b, Kpad,
+                   reinterpret_cast<__nv_bfloat16*>(hi), reinterpret_cast<__nv_bfloat16*>(lo));
 }
 
 cudaError_t launch_cls_rows(const float* cls, const float* pos, int b, float* x, cudaStream_t s) {

@@ -11,15 +11,11 @@ import torch
 
 from . import _lib
 from ._lib import (GpCandidates, GpConfig, GpMatches, GpPredictions, GpRansacOut, LAYOUT_CHANNEL_MAJOR,
-                   LAYOUT_PATCH_MAJOR, LAYOUT_VIT_TOKENS, PRECISION_BF16, PRECISION_FP32_SPLIT, check)
+                   LAYOUT_PATCH_MAJOR, LAYOUT_VIT_TOKENS, PRECISION_BF16, PRECISION_FP32_SPLIT, check, ptr)
 
 P = 256
 C_AE = 1024
 C_IST = 256
-
-
-def _ptr(t: Optional[torch.Tensor]) -> Optional[int]:
-    return None if t is None else t.data_ptr()
 
 
 def _f32(t: torch.Tensor, device) -> torch.Tensor:
@@ -71,11 +67,7 @@ class Engine:
                  patch_size: int = 14, precision: str = "fp32_split", shard_rank: int = 0, shard_world: int = 1,
                  num_templates_global: Optional[int] = None, ist_bank_global: bool = False):
         self.lib = _lib.load()
-        self.device = torch.device(device)
-        if self.device.type != "cuda":
-            raise _lib.GigaPoseNativeError("gigapose_b200 runs on CUDA devices only (no CPU fallback)")
-        if self.device.index is None:
-            self.device = torch.device("cuda", torch.cuda.current_device())
+        self.device = _lib.cuda_device(device, "gigapose_b200 runs")
         self.k = int(k)
         self.O, self.T, self.max_batch = int(num_objects), int(num_templates), int(max_batch)
         self.T_global = int(num_templates_global if num_templates_global is not None else num_templates)
@@ -94,14 +86,10 @@ class Engine:
         bank_b, ws_b = C.c_size_t(), C.c_size_t()
         check(self.lib.gp_query_sizes(C.byref(cfg), C.byref(bank_b), C.byref(ws_b)))
         self.bank_bytes, self.workspace_bytes = bank_b.value, ws_b.value
-        with torch.cuda.device(self.device):
-            # +1 KiB so the carved base can be aligned to 1024 B whatever the allocator returns
-            self._bank_mem = torch.empty(self.bank_bytes + 1024, dtype=torch.uint8, device=self.device)
-            self._ws_mem = torch.empty(self.workspace_bytes + 1024, dtype=torch.uint8, device=self.device)
-            self._bank_mem.zero_()
-        al = lambda t: (t.data_ptr() + 1023) // 1024 * 1024
+        self._bank_mem, self._bank = _lib.aligned_buffer(self.bank_bytes, self.device, zero=True)
+        self._ws_mem, ws = _lib.aligned_buffer(self.workspace_bytes, self.device)
         h = C.c_void_p()
-        check(self.lib.gp_create(C.byref(cfg), al(self._bank_mem), al(self._ws_mem), C.byref(h)))
+        check(self.lib.gp_create(C.byref(cfg), self._bank.data_ptr(), ws.data_ptr(), C.byref(h)))
         self._h = h
         self._keep = []          # tensors whose device pointers the library retains
         self._B = 0
@@ -157,8 +145,8 @@ class Engine:
     BANK_FORMAT = 1
 
     def _bank_view(self) -> torch.Tensor:
-        off = (-self._bank_mem.data_ptr()) % 1024
-        return self._bank_mem[off:off + self.bank_bytes]
+        """The bank as the library carves it: `bank_bytes` bytes from the 1024-aligned base."""
+        return self._bank
 
     def _bank_header(self) -> dict:
         c = self.cfg
@@ -248,7 +236,7 @@ class Engine:
     @staticmethod
     def _cand_struct(c) -> GpCandidates:
         return GpCandidates(c["score"].data_ptr(), c["id"].data_ptr(), c["pts_score"].data_ptr(), c["idx"].data_ptr(),
-                            c["valid"].data_ptr(), _ptr(c.get("rel_scale")), _ptr(c.get("rel_inplane")))
+                            c["valid"].data_ptr(), ptr(c.get("rel_scale")), ptr(c.get("rel_inplane")))
 
     def sim_topk(self) -> Dict[str, torch.Tensor]:
         """LocalSimilarity.test on the staged queries against the resident bank (single GPU)."""
@@ -273,7 +261,7 @@ class Engine:
         if gathered.get("rel_scale") is not None:
             rs = self._empty((B, self.k, P), torch.float32)
             ri = self._empty((B, self.k, P, 2), torch.float32)
-        check(self.lib.gp_topk_merge(self._h, B, G, C.byref(cs), rank_stride_bytes, C.byref(ms), _ptr(rs), _ptr(ri),
+        check(self.lib.gp_topk_merge(self._h, B, G, C.byref(cs), rank_stride_bytes, C.byref(ms), ptr(rs), ptr(ri),
                                      self.stream))
         return (m, rs, ri) if rs is not None else m
 

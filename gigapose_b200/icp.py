@@ -10,7 +10,7 @@ import ctypes as C
 import torch
 
 from . import _lib
-from ._lib import GpIcpDebug, GpIcpParams, check
+from ._lib import GpIcpDebug, GpIcpParams, check, ptr
 from .render import _device_mesh, render_chunk
 
 STATUS_NAMES = {_lib.ICP_OK: "ok", _lib.ICP_TOO_FEW_POINTS: "too few points", _lib.ICP_DEGENERATE: "degenerate",
@@ -21,10 +21,6 @@ DEFAULTS = dict(unit_per_m=1000.0, min_points=1000, num_levels=4, max_iters=100,
 WORKSPACE_BYTES = 1 << 30          # renders + ICP scratch per chunk of hypotheses: ~20 MB per 640 x 480 hypothesis
 
 
-def _ptr(x):
-    return x.data_ptr() if x is not None else None
-
-
 def make_params(debug=None, **params) -> GpIcpParams:
     unknown = set(params) - set(DEFAULTS)
     if unknown:
@@ -32,7 +28,7 @@ def make_params(debug=None, **params) -> GpIcpParams:
     p = dict(DEFAULTS, **params)
     out = GpIcpParams(**p)
     if debug:
-        out.debug = GpIcpDebug(**{k: v if isinstance(v, int) else _ptr(v) for k, v in debug.items()})
+        out.debug = GpIcpDebug(**{k: v if isinstance(v, int) else ptr(v) for k, v in debug.items()})
     return out
 
 
@@ -91,7 +87,7 @@ def refine_rendered(depth, K, frame_idx, rendered, boxes, poses, masks, workspac
     residual = torch.empty(n, device=dev)
     fitness = torch.empty(n, device=dev)
     p = make_params(debug, **params)
-    check(_lib.load().gp_icp_refine(F, n, H, W, frame_idx.data_ptr(), _ptr(masks), rendered.data_ptr(), boxes.data_ptr(),
+    check(_lib.load().gp_icp_refine(F, n, H, W, frame_idx.data_ptr(), ptr(masks), rendered.data_ptr(), boxes.data_ptr(),
                                     poses.data_ptr(), K.data_ptr(), C.byref(p), out.data_ptr(), status.data_ptr(),
                                     residual.data_ptr(), fitness.data_ptr(), workspace.data_ptr(),
                                     torch.cuda.current_stream(dev).cuda_stream))

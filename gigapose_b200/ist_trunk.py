@@ -67,9 +67,7 @@ def _version_key(resnet):
 class NativeISTTrunk:
     def __init__(self, resnet, device, max_crops: int = 32, precision: str = "fp32_split"):
         self.lib = _lib.load()
-        self.device = torch.device(device)
-        if self.device.type != "cuda":
-            raise _lib.GigaPoseNativeError("the IST trunk kernels run on CUDA devices only (no CPU fallback)")
+        self.device = _lib.cuda_device(device, "the IST trunk kernels run")
         if not supports(resnet):
             raise _lib.GigaPoseNativeError("the IST trunk kernels are specialised for the shipped ResNet geometry")
         self.max_crops = max_crops
@@ -77,16 +75,14 @@ class NativeISTTrunk:
             self.weights = folded_convs_in_abi_order(resnet, self.device)     # biases referenced in place: keep alive
         wb, sb = C.c_size_t(), C.c_size_t()
         check(self.lib.gp_ist_trunk_query_sizes(max_crops, C.byref(wb), C.byref(sb)))
-        with torch.cuda.device(self.device):
-            self._wmem = torch.empty(wb.value + 1024, dtype=torch.uint8, device=self.device)
-            self._smem = torch.zeros(sb.value + 1024, dtype=torch.uint8, device=self.device)
-        al = lambda t: (t.data_ptr() + 1023) // 1024 * 1024
-        arr = (ConvWeights * NUM_CONVS)(*[ConvWeights(w.data_ptr(), b.data_ptr() if b is not None else None)
+        self._wmem, wview = _lib.aligned_buffer(wb.value, self.device)
+        self._smem, sview = _lib.aligned_buffer(sb.value, self.device, zero=True)
+        arr = (ConvWeights * NUM_CONVS)(*[ConvWeights(w.data_ptr(), _lib.ptr(b))
                                           for w, b in self.weights])
         h = C.c_void_p()
         prec = {"fp32_split": _lib.PRECISION_FP32_SPLIT, "bf16": _lib.PRECISION_BF16}[precision]
-        check(self.lib.gp_ist_trunk_create(self.device.index or 0, max_crops, prec, C.cast(arr, C.c_void_p), al(self._wmem),
-                                           al(self._smem), torch.cuda.current_stream(self.device).cuda_stream, C.byref(h)))
+        check(self.lib.gp_ist_trunk_create(self.device.index, max_crops, prec, C.cast(arr, C.c_void_p), wview.data_ptr(),
+                                           sview.data_ptr(), torch.cuda.current_stream(self.device).cuda_stream, C.byref(h)))
         self._h = h
         self.precision = precision
 

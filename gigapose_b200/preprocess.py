@@ -9,7 +9,7 @@ from typing import Optional, Sequence
 import torch
 
 from . import _lib
-from ._lib import check
+from ._lib import check, ptr
 
 CLIP_MEAN = (0.48145466, 0.4578275, 0.40821073)
 CLIP_STD = (0.26862954, 0.26130258, 0.27577711)
@@ -48,7 +48,6 @@ def crop_resize_pad(xyxy_boxes: torch.Tensor, images: torch.Tensor, target_size:
     out = torch.empty(n, C, T, T, device=dev)
     out_mask = torch.empty(n, T, T, device=dev) if m is not None else None
     M = torch.empty(n, 3, 3, device=dev)
-    ptr = lambda t: t.data_ptr() if t is not None else None
     with torch.cuda.device(dev):
         check(lib.gp_crop_resize_pad(n, C, H, W, T, images.data_ptr(), ptr(idx), boxes.data_ptr(), ptr(m), float(in_div),
                                      ptr(sub), ptr(div), out.data_ptr(), ptr(out_mask), M.data_ptr(),

@@ -12,7 +12,7 @@ import numpy as np
 import torch
 
 from . import _lib
-from ._lib import check
+from ._lib import check, ptr
 
 # the template camera of the reference (call_panda3d.py:45-47): the LINEMOD focal lengths with the principal point at
 # the image centre of 640 x 480
@@ -184,19 +184,15 @@ def _device_mesh(mesh, device):
     return out
 
 
-def _ptr(x):
-    return x.data_ptr() if x is not None else None
-
-
 def render_chunk(dm, poses, K, H, W, z_near, workspace, rgba, depth, boxes):
     """One gp_render_templates call on device tensors (dm from _device_mesh); enqueued on the current stream."""
     lib = _lib.load()
     tex = dm["texture"]
-    check(lib.gp_render_templates(poses.shape[0], H, W, dm["vertices"].shape[0], _ptr(dm["vertices"]), dm["faces"].shape[0],
-                                  _ptr(dm["faces"]), _ptr(dm["vertex_color"]), _ptr(dm["face_uv"]), _ptr(tex),
+    check(lib.gp_render_templates(poses.shape[0], H, W, dm["vertices"].shape[0], ptr(dm["vertices"]), dm["faces"].shape[0],
+                                  ptr(dm["faces"]), ptr(dm["vertex_color"]), ptr(dm["face_uv"]), ptr(tex),
                                   tex.shape[0] if tex is not None else 0, tex.shape[1] if tex is not None else 0,
-                                  _ptr(dm["constant_color"]), poses.data_ptr(), K.data_ptr(), float(z_near),
-                                  workspace.data_ptr(), rgba.data_ptr(), _ptr(depth), boxes.data_ptr(),
+                                  ptr(dm["constant_color"]), poses.data_ptr(), K.data_ptr(), float(z_near),
+                                  workspace.data_ptr(), rgba.data_ptr(), ptr(depth), boxes.data_ptr(),
                                   torch.cuda.current_stream(poses.device).cuda_stream))
 
 

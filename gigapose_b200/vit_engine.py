@@ -49,23 +49,19 @@ def _version_key(m):
 class NativeViT:
     def __init__(self, model, device, max_crops: int = 64, precision: str = "fp32_split"):
         self.lib = _lib.load()
-        self.device = torch.device(device)
-        if self.device.type != "cuda":
-            raise _lib.GigaPoseNativeError("the ViT kernels run on CUDA devices only (no CPU fallback)")
+        self.device = _lib.cuda_device(device, "the ViT kernels run")
         self.depth = len(model.blocks)
         self.max_crops = max_crops
         self.weights = _params_in_abi_order(model, self.device)          # kept alive: referenced in place
         wb, sb = C.c_size_t(), C.c_size_t()
         check(self.lib.gp_vit_query_sizes(self.depth, max_crops, C.byref(wb), C.byref(sb)))
-        with torch.cuda.device(self.device):
-            self._wmem = torch.empty(wb.value + 1024, dtype=torch.uint8, device=self.device)
-            self._smem = torch.empty(sb.value + 1024, dtype=torch.uint8, device=self.device)
-        al = lambda t: (t.data_ptr() + 1023) // 1024 * 1024
+        self._wmem, wview = _lib.aligned_buffer(wb.value, self.device)
+        self._smem, sview = _lib.aligned_buffer(sb.value, self.device)
         arr = (C.c_void_p * len(self.weights))(*[w.data_ptr() for w in self.weights])
         h = C.c_void_p()
         prec = {"fp32_split": _lib.PRECISION_FP32_SPLIT, "bf16": _lib.PRECISION_BF16}[precision]
-        check(self.lib.gp_vit_create(self.device.index or 0, self.depth, max_crops, prec, arr, al(self._wmem),
-                                     al(self._smem), torch.cuda.current_stream(self.device).cuda_stream, C.byref(h)))
+        check(self.lib.gp_vit_create(self.device.index, self.depth, max_crops, prec, arr, wview.data_ptr(), sview.data_ptr(),
+                                     torch.cuda.current_stream(self.device).cuda_stream, C.byref(h)))
         self._h = h
         self.precision = precision
 

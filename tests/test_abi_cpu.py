@@ -71,6 +71,20 @@ def test_product_code_never_imports_the_oracle():
     assert not offenders, offenders
 
 
+def test_every_kernel_launch_goes_through_the_counting_launcher():
+    """gp_launch_count() (bench.py's `gpu_launches`) is kept by the one launcher in csrc/runtime.cu, so it cannot drift
+    from the kernels really launched: no `<<<...>>>` launch in any source, and one place increments the counter."""
+    csrc = os.path.join(ROOT, "gigapose_b200", "csrc")
+    chevrons, increments = [], []
+    for f in sorted(os.listdir(csrc)):
+        txt = open(os.path.join(csrc, f)).read()
+        if "<<<" in txt:
+            chevrons.append(f)
+        increments += [f] * len(re.findall(r"g_launches\s*(?:\+\+|\+=|\.fetch_add)|\+\+\s*g_launches", txt))
+    assert not chevrons, chevrons
+    assert increments == ["runtime.cu"], increments
+
+
 def test_abi_v2_config_and_argument_checks_need_no_gpu(lib):
     """ABI 2: the replicated IST bank is sized by `ist_bank_global`; the multi-GPU and helper entry points reject bad
     arguments through the status channel without touching a device."""
