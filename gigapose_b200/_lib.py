@@ -18,6 +18,8 @@ LAYOUT_VIT_TOKENS = 2
 PRECISION_FP32_SPLIT = 0
 PRECISION_BF16 = 1
 MAX_NUM_TEMPLATES = 12032      # GP_MAX_NUM_TEMPLATES: largest num_templates per handle
+BOP_MAX_TAU = 16               # GP_BOP_MAX_TAU
+BOP_MAX_OBJECTS = 256          # GP_BOP_MAX_OBJECTS
 
 
 class GpConfig(C.Structure):
@@ -132,6 +134,14 @@ SYMBOLS = {
     "gp_render_templates": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p,
                                       C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
                                       C.c_float, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "gp_render_depth": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p,
+                                  C.c_void_p, C.c_float, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "gp_bop_vsd": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p,
+                             C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_float,
+                             C.c_int, C.POINTER(C.c_float), C.c_void_p, C.c_void_p, C.c_void_p]),
+    "gp_bop_mssd_mspd": (C.c_int, [C.c_int, C.c_int, C.c_void_p, C.POINTER(C.c_int32), C.c_void_p, C.POINTER(C.c_int32),
+                                   C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                   C.c_void_p, C.c_void_p]),
     "gp_icp_query_sizes": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_size_t)]),
     "gp_icp_prepare_scene": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_float, C.c_void_p,
                                        C.c_void_p]),

@@ -1,0 +1,478 @@
+"""BOP 2019 pose-error evaluation on the GPU (row f7): VSD, MSSD, MSPD and the average recalls, in place of the external
+BOP toolkit's eval_bop19_pose.py that the reference shells out to (src/scripts/eval_bop.py:16-38).
+
+Estimates and ground truths are rendered with `gp_render_depth` (one depth sample at each pixel centre), the per-pixel
+VSD counts and the symmetry-aware vertex distances run in csrc/bop_eval.cu (whose header comment states the fp32
+contract), and the matching into recalls runs here in numpy.  Usage:
+
+    python -m gigapose_b200.bop_eval --results X.csv --dataset-dir D [--split test] [--out DIR]
+"""
+from __future__ import annotations
+
+import argparse
+import ctypes as C
+import json
+import os
+
+import numpy as np
+import torch
+
+from . import _lib
+from ._lib import check
+from .render import read_ply
+
+# Defaults of the BOP 2019/2020 methodology: VSD from Hodan et al., "BOP: Benchmark for 6D Object Pose Estimation"
+# (ECCV 2018); MSSD, MSPD and the AR from Hodan et al., "BOP Challenge 2020 on 6D Object Localization" (ECCV 2020
+# workshops).  They are taken from those papers; they could not be checked against the toolkit's own configuration.
+DELTA = 15.0                    # VSD visibility tolerance, model unit (mm)
+DELTA_ITODD = 5.0
+TAUS = tuple(round(0.05 * i, 2) for i in range(1, 11))          # VSD misalignment tolerance, x diameter
+THETA_VSD = TAUS                                                 # VSD correctness thresholds
+THETA_MSSD = TAUS                                                # x diameter
+THETA_MSPD = tuple(5.0 * i for i in range(1, 11))                # x r, r = image width / 640
+MAX_SYM_DISC_STEP = 0.01        # continuous symmetries: the farthest vertex moves <= 1 % of the diameter per step
+VISIB_GT_MIN = 0.1              # ground truths less visible than this are neither targets nor matchable
+Z_NEAR = 10.0                   # renders: near plane, model unit
+WORKSPACE_BYTES = 1 << 30       # device memory per chunk of images: measured depth, renders and the render keys
+
+
+class BopEvalError(ValueError):
+    pass
+
+
+# ---------------------------------------------------------------------------------------------------- readers
+def _json(path):
+    if not os.path.exists(path):
+        raise BopEvalError(f"{path} not found")
+    with open(path) as f:
+        return json.load(f)
+
+
+def load_scene(dataset_dir, split, scene_id):
+    """-> dict(gt={im: [dict(R [3,3], t [3], obj_id)]}, visib={im: [visib_fract]}, K={im: [3,3]},
+    depth_scale={im: float}) from scene_gt.json, scene_gt_info.json and scene_camera.json."""
+    d = os.path.join(dataset_dir, split, f"{scene_id:06d}")
+    gt = _json(os.path.join(d, "scene_gt.json"))
+    info = _json(os.path.join(d, "scene_gt_info.json"))
+    cam = _json(os.path.join(d, "scene_camera.json"))
+    out = dict(gt={}, visib={}, K={}, depth_scale={})
+    for im, insts in gt.items():
+        out["gt"][int(im)] = [dict(R=np.asarray(g["cam_R_m2c"], np.float64).reshape(3, 3),
+                                   t=np.asarray(g["cam_t_m2c"], np.float64).reshape(3), obj_id=int(g["obj_id"]))
+                              for g in insts]
+        out["visib"][int(im)] = [float(i["visib_fract"]) for i in info[im]]
+    for im, c in cam.items():
+        out["K"][int(im)] = np.asarray(c["cam_K"], np.float64).reshape(3, 3)
+        out["depth_scale"][int(im)] = float(c.get("depth_scale", 1.0))
+    return out
+
+
+def load_depth(dataset_dir, split, scene_id, im_id, depth_scale):
+    """16-bit PNG depth x depth_scale -> f32 [H,W] in the model unit (0 = missing)."""
+    from PIL import Image
+    path = os.path.join(dataset_dir, split, f"{scene_id:06d}", "depth", f"{im_id:06d}.png")
+    if not os.path.exists(path):
+        raise BopEvalError(f"{path} not found: VSD needs the depth images, and this dataset or split has none")
+    with Image.open(path) as im:
+        raw = np.asarray(im)
+    return (raw.astype(np.float64) * depth_scale).astype(np.float32)
+
+
+def models_dir(dataset_dir):
+    """models_eval/ (the evaluation models of a BOP dataset) when present, else models/."""
+    d = os.path.join(dataset_dir, "models_eval")
+    return d if os.path.isdir(d) else os.path.join(dataset_dir, "models")
+
+
+def load_models_info(mdir):
+    """-> {obj_id: dict(diameter, symmetries_discrete [k,4,4], symmetries_continuous [(axis [3], offset [3])])}."""
+    info = _json(os.path.join(mdir, "models_info.json"))
+    out = {}
+    for k, v in info.items():
+        out[int(k)] = dict(diameter=float(v["diameter"]),
+                           symmetries_discrete=[np.asarray(s, np.float64).reshape(4, 4)
+                                                for s in v.get("symmetries_discrete", [])],
+                           symmetries_continuous=[(np.asarray(s["axis"], np.float64), np.asarray(s["offset"], np.float64))
+                                                  for s in v.get("symmetries_continuous", [])])
+    return out
+
+
+def load_targets(dataset_dir, name="test_targets_bop19.json"):
+    """-> list of dict(scene_id, im_id, obj_id, inst_count)."""
+    return [dict(scene_id=int(t["scene_id"]), im_id=int(t["im_id"]), obj_id=int(t["obj_id"]),
+                 inst_count=int(t["inst_count"])) for t in _json(os.path.join(dataset_dir, name))]
+
+
+def load_results(results):
+    """A csv path (`src.utils.inout.load_bop_results`) or a list of dicts in that format."""
+    if isinstance(results, (str, os.PathLike)):
+        from src.utils.inout import load_bop_results
+        return load_bop_results(results)
+    return list(results)
+
+
+# ---------------------------------------------------------------------------------------------------- symmetries
+def _axis_rotation(axis, angle):
+    a = np.asarray(axis, np.float64) / np.linalg.norm(axis)
+    k = np.array([[0, -a[2], a[1]], [a[2], 0, -a[0]], [-a[1], a[0], 0]])
+    return np.eye(3) + np.sin(angle) * k + (1 - np.cos(angle)) * (k @ k)
+
+
+def symmetry_transforms(info, max_sym_disc_step=MAX_SYM_DISC_STEP):
+    """Symmetry transforms [S,4,4] (fp64) of an object.  Discrete: the identity, then each declared discrete symmetry D.
+    Continuous: each (axis a, offset o) becomes n = ceil(pi / max_sym_disc_step) rotations C_k by k * 2 pi / n,
+    k = 0 .. n - 1, about the line through o along a (x -> R_k (x - o) + o), so that the vertex farthest from the axis
+    (at most half a diameter away) moves at most max_sym_disc_step x diameter between two steps.  With continuous
+    symmetries the transforms are the compositions C_k D (D applied first), discrete-major: for each D in the order
+    above, every C_k of the first continuous symmetry, then of the next."""
+    disc = [np.eye(4)] + [np.asarray(s, np.float64).reshape(4, 4) for s in info.get("symmetries_discrete", [])]
+    cont = []
+    for axis, offset in info.get("symmetries_continuous", []):
+        n = int(np.ceil(np.pi / max_sym_disc_step))
+        o = np.asarray(offset, np.float64).reshape(3)
+        for k in range(n):
+            T = np.eye(4)
+            T[:3, :3] = _axis_rotation(axis, k * 2.0 * np.pi / n)
+            T[:3, 3] = o - T[:3, :3] @ o
+            cont.append(T)
+    if not cont:
+        return np.stack(disc)
+    return np.stack([c @ d for d in disc for c in cont])
+
+
+# ---------------------------------------------------------------------------------------------------- matching
+def match_group(err, valid, thresholds):
+    """Greedy matching of one (image, object): err [n_est, n_gt] with the estimates in descending score order, valid
+    [n_gt] (matchable ground truths), thresholds [T] -> matched ground truths per threshold [T].  Each estimate in turn
+    takes the unmatched valid ground truth with the smallest error strictly below the threshold (the lowest index on a
+    tie)."""
+    err = np.asarray(err, np.float64).reshape(-1, len(valid))
+    th = np.asarray(thresholds, np.float64)
+    taken = np.zeros((len(th), err.shape[1]), bool)
+    for row in err:
+        cand = valid[None] & ~taken & (row[None] < th[:, None])
+        j = np.argmin(np.where(cand, row[None], np.inf), axis=1)
+        has = cand.any(1)
+        taken[np.nonzero(has)[0], j[has]] = True
+    return taken.sum(1)
+
+
+def recalls(groups, n_targets, taus=TAUS, theta_vsd=THETA_VSD, theta_mssd=THETA_MSSD, theta_mspd=THETA_MSPD, r=1.0):
+    """groups: list of dict(vsd [n_est,n_gt,n_tau], mssd / mspd [n_est,n_gt], valid [n_gt], diameter) -> recall
+    arrays: vsd [n_tau, n_theta], mssd [n_theta], mspd [n_theta] (matched targets / n_targets)."""
+    m_vsd = np.zeros((len(taus), len(theta_vsd)))
+    m_mssd, m_mspd = np.zeros(len(theta_mssd)), np.zeros(len(theta_mspd))
+    for g in groups:
+        if g["mssd"].shape[0] == 0:
+            continue
+        for t in range(len(taus)):
+            m_vsd[t] += match_group(g["vsd"][:, :, t], g["valid"], theta_vsd)
+        m_mssd += match_group(g["mssd"], g["valid"], np.asarray(theta_mssd) * g["diameter"])
+        m_mspd += match_group(g["mspd"], g["valid"], np.asarray(theta_mspd) * r)
+    n = max(n_targets, 1)
+    return dict(vsd=m_vsd / n, mssd=m_mssd / n, mspd=m_mspd / n)
+
+
+# ---------------------------------------------------------------------------------------------------- set-up
+def prepare(results, dataset_dir, split="test", targets_name="test_targets_bop19.json"):
+    """Host side: reads the dataset, keeps the top inst_count estimates per target by score and lists every
+    (estimate, ground truth) pair of the same object in an image.  -> dict with `images` [(scene, im)], `targets`,
+    per-image estimates / ground truths and `pairs`."""
+    results = load_results(results)
+    targets = load_targets(dataset_dir, targets_name)
+    mdir = models_dir(dataset_dir)
+    info = load_models_info(mdir)
+    by_key = {}
+    for i, res in enumerate(results):
+        by_key.setdefault((res["scene_id"], res["im_id"], res["obj_id"]), []).append(i)
+    scenes, images = {}, []
+    groups = []                      # one per target: (scene, im, obj), kept estimate ids, gt instance ids, valid
+    for t in targets:
+        s, im, o = t["scene_id"], t["im_id"], t["obj_id"]
+        if o not in info:
+            raise BopEvalError(f"object {o} of a target is not in {mdir}/models_info.json")
+        if s not in scenes:
+            scenes[s] = load_scene(dataset_dir, split, s)
+        sc = scenes[s]
+        if im not in sc["gt"] or im not in sc["K"]:
+            raise BopEvalError(f"target image {s}/{im} is not in scene_gt.json / scene_camera.json")
+        if (s, im) not in images:
+            images.append((s, im))
+        ests = by_key.get((s, im, o), [])
+        ests = sorted(ests, key=lambda i: -results[i]["score"])[:t["inst_count"]]      # stable: csv order on ties
+        gts = [k for k, g in enumerate(sc["gt"][im]) if g["obj_id"] == o]
+        valid = np.array([sc["visib"][im][k] >= VISIB_GT_MIN for k in gts], bool)
+        groups.append(dict(scene_id=s, im_id=im, obj_id=o, est=ests, gt=gts, valid=valid))
+    return dict(results=results, targets=targets, groups=groups, images=images, scenes=scenes, info=info, mdir=mdir,
+                dataset_dir=dataset_dir, split=split)
+
+
+# ---------------------------------------------------------------------------------------------------- device stages
+def _pose(R, t):
+    T = np.eye(4)
+    T[:3, :3] = np.asarray(R, np.float64).reshape(3, 3)
+    T[:3, 3] = np.asarray(t, np.float64).reshape(3)
+    return T
+
+
+class _Stages:
+    """CUDA events around each stage of each chunk; milliseconds summed per stage after a synchronise."""
+
+    def __init__(self, enabled):
+        self.enabled, self.marks = enabled, []
+
+    def mark(self, name):
+        if not self.enabled:
+            return None
+        ev = (torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True))
+        ev[0].record()
+        self.marks.append((name, ev))
+        return ev[1]
+
+    def totals(self):
+        torch.cuda.synchronize()
+        out = {}
+        for name, (a, b) in self.marks:
+            out[name] = out.get(name, 0.0) + a.elapsed_time(b)
+        return out
+
+
+def render_depth(dm, poses, K, H, W, z_near, workspace, depth, boxes):
+    """One gp_render_depth call on device tensors (dm from icp.device_meshes); enqueued on the current stream."""
+    check(_lib.load().gp_render_depth(poses.shape[0], H, W, dm["vertices"].shape[0], dm["vertices"].data_ptr(),
+                                      dm["faces"].shape[0], dm["faces"].data_ptr(), poses.data_ptr(), K.data_ptr(),
+                                      float(z_near), workspace.data_ptr(), depth.data_ptr(), boxes.data_ptr(),
+                                      torch.cuda.current_stream(poses.device).cuda_stream))
+
+
+def vsd(depth_test, K, frame_idx, est_depth, est_boxes, est_idx, gt_depth, gt_boxes, gt_idx, diameter, delta, taus):
+    """gp_bop_vsd on device tensors -> counts i32 [n, 2 + n_tau], errors f32 [n, n_tau]."""
+    n, F, H, W = frame_idx.shape[0], depth_test.shape[0], depth_test.shape[1], depth_test.shape[2]
+    counts = torch.empty(n, 2 + len(taus), dtype=torch.int32, device=depth_test.device)
+    errors = torch.empty(n, len(taus), device=depth_test.device)
+    tau = (C.c_float * len(taus))(*taus)
+    check(_lib.load().gp_bop_vsd(n, F, H, W, depth_test.data_ptr(), K.data_ptr(), frame_idx.data_ptr(),
+                                 est_depth.shape[0], est_depth.data_ptr(), est_boxes.data_ptr(), est_idx.data_ptr(),
+                                 gt_depth.shape[0], gt_depth.data_ptr(), gt_boxes.data_ptr(), gt_idx.data_ptr(),
+                                 diameter.data_ptr(), float(delta), len(taus), tau, counts.data_ptr(), errors.data_ptr(),
+                                 torch.cuda.current_stream(depth_test.device).cuda_stream))
+    return counts, errors
+
+
+def mssd_mspd(obj_idx, vertex_offsets, vertices, sym_offsets, syms, K, frame_idx, pose_est, pose_gt):
+    """gp_bop_mssd_mspd on device tensors (offsets are host int sequences) -> mssd, mspd f32 [n]."""
+    n = obj_idx.shape[0]
+    mssd = torch.empty(n, device=vertices.device)
+    mspd = torch.empty(n, device=vertices.device)
+    vo = (C.c_int32 * len(vertex_offsets))(*vertex_offsets)
+    so = (C.c_int32 * len(sym_offsets))(*sym_offsets)
+    check(_lib.load().gp_bop_mssd_mspd(n, len(vertex_offsets) - 1, obj_idx.data_ptr(), vo, vertices.data_ptr(), so,
+                                       syms.data_ptr(), K.shape[0], K.data_ptr(), frame_idx.data_ptr(),
+                                       pose_est.data_ptr(), pose_gt.data_ptr(), mssd.data_ptr(), mspd.data_ptr(),
+                                       torch.cuda.current_stream(vertices.device).cuda_stream))
+    return mssd, mspd
+
+
+def compute_errors(setup, device="cuda", delta=None, taus=TAUS, z_near=Z_NEAR, stage_ms=None):
+    """Per-pair errors of every (kept estimate, ground truth of its object) pair on the device, one chunk of images at a
+    time within WORKSPACE_BYTES.  -> dict of numpy arrays over the pairs: group (target index), est (result index),
+    gt (instance index in scene_gt), vsd [n, n_tau], vsd_counts [n, 2 + n_tau], mssd, mspd.  `stage_ms` (a dict)
+    receives the summed milliseconds of the stages renders / vsd / mssd_mspd, from CUDA events."""
+    from .icp import device_meshes
+    device = _lib.cuda_device(device, "BOP evaluation")
+    if not 1 <= len(taus) <= _lib.BOP_MAX_TAU:
+        raise BopEvalError(f"between 1 and {_lib.BOP_MAX_TAU} VSD tolerances, got {len(taus)}")
+    if delta is None:
+        itodd = os.path.basename(os.path.normpath(setup["dataset_dir"])) == "itodd"
+        delta = DELTA_ITODD if itodd else DELTA
+    results, groups, scenes, info = setup["results"], setup["groups"], setup["scenes"], setup["info"]
+    obj_ids = sorted({g["obj_id"] for g in groups})
+    if len(obj_ids) > _lib.BOP_MAX_OBJECTS:
+        raise BopEvalError(f"at most {_lib.BOP_MAX_OBJECTS} objects per evaluation")
+    oidx = {o: i for i, o in enumerate(obj_ids)}
+    out = dict(group=[], est=[], gt=[], vsd=[], vsd_counts=[], mssd=[], mspd=[])
+    if not obj_ids:
+        return {k: np.zeros((0,)) for k in out}
+    stages = _Stages(stage_ms is not None)
+    meshes = [read_ply(os.path.join(setup["mdir"], f"obj_{o:06d}.ply")) for o in obj_ids]
+    with torch.cuda.device(device):
+        dms = device_meshes(meshes, device)
+        vo = np.concatenate([[0], np.cumsum([len(m["vertices"]) for m in meshes])]).astype(np.int32)
+        vertices = torch.as_tensor(np.concatenate([m["vertices"] for m in meshes]), device=device).contiguous()
+        sym = [symmetry_transforms(info[o]) for o in obj_ids]
+        so = np.concatenate([[0], np.cumsum([len(s) for s in sym])]).astype(np.int32)
+        syms = torch.as_tensor(np.concatenate(sym), dtype=torch.float32, device=device).contiguous()
+        diam = {o: info[o]["diameter"] for o in obj_ids}
+        by_image = {}
+        for gi, g in enumerate(groups):
+            by_image.setdefault((g["scene_id"], g["im_id"]), []).append(gi)
+        # chunks of images: measured depth plus every render of the chunk within half of the budget
+        first = setup["images"][0]
+        H, W = load_depth(setup["dataset_dir"], setup["split"], first[0], first[1],
+                          scenes[first[0]]["depth_scale"][first[1]]).shape
+        plane = 4 * H * W
+        chunks, cur, cur_bytes = [], [], 0
+        for key in setup["images"]:
+            b = plane * (1 + sum(len(groups[gi]["est"]) + len(groups[gi]["gt"]) for gi in by_image[key]))
+            if cur and cur_bytes + b > WORKSPACE_BYTES // 2:
+                chunks.append(cur)
+                cur, cur_bytes = [], 0
+            cur.append(key)
+            cur_bytes += b
+        chunks.append(cur)
+        key_views = max(1, WORKSPACE_BYTES // 2 // (8 * H * W))
+        keys_ws = torch.empty(key_views * 8 * H * W, dtype=torch.uint8, device=device)
+        for chunk in chunks:
+            depth_np, K_np = [], []
+            renders = []               # (object, pose [4,4], frame) of every estimate, then every ground truth
+            pair_rows = []             # (group, est id, gt id, frame, est render, gt render)
+            for f, (s, im) in enumerate(chunk):
+                sc = scenes[s]
+                d = load_depth(setup["dataset_dir"], setup["split"], s, im, sc["depth_scale"][im])
+                if d.shape != (H, W):
+                    raise BopEvalError(f"depth of {s}/{im} is {d.shape}, the first image's is {(H, W)}")
+                depth_np.append(d)
+                K_np.append(sc["K"][im])
+                for gi in by_image[(s, im)]:
+                    g = groups[gi]
+                    er = []
+                    for e in g["est"]:
+                        er.append(len(renders))
+                        renders.append((g["obj_id"], _pose(results[e]["R"], results[e]["t"]), f))
+                    gr = []
+                    for k in g["gt"]:
+                        gr.append(len(renders))
+                        renders.append((g["obj_id"], _pose(sc["gt"][im][k]["R"], sc["gt"][im][k]["t"]), f))
+                    for a, e in enumerate(g["est"]):
+                        for b, k in enumerate(g["gt"]):
+                            pair_rows.append((gi, e, k, f, er[a], gr[b]))
+            if not pair_rows:
+                continue
+            done = stages.mark("renders")
+            depth_test = torch.as_tensor(np.stack(depth_np), device=device)
+            K = torch.as_tensor(np.stack(K_np), dtype=torch.float32, device=device).contiguous()
+            n_r = len(renders)
+            rdepth = torch.empty(n_r, H, W, device=device)
+            rboxes = torch.empty(n_r, 4, dtype=torch.int64, device=device)
+            poses = torch.as_tensor(np.stack([r[1] for r in renders]), dtype=torch.float32, device=device)
+            batches = {}
+            for i, (o, _, f) in enumerate(renders):          # one call per (object, K) shares the mesh and K
+                batches.setdefault((o, K_np[f].astype(np.float32).tobytes()), []).append(i)
+            for (o, _), idx in batches.items():
+                Kf = K[renders[idx[0]][2]].contiguous()
+                for s0 in range(0, len(idx), key_views):
+                    sel = torch.as_tensor(idx[s0:s0 + key_views], device=device)
+                    d = torch.empty(len(sel), H, W, device=device)
+                    b = torch.empty(len(sel), 4, dtype=torch.int64, device=device)
+                    render_depth(dms[oidx[o]], poses[sel].contiguous(), Kf, H, W, z_near, keys_ws, d, b)
+                    rdepth[sel], rboxes[sel] = d, b
+            if done is not None:
+                done.record()
+            rows = np.array(pair_rows, np.int64)
+            col = lambda j: torch.as_tensor(rows[:, j].astype(np.int32), device=device)
+            fi, ei, gi_ = col(3), col(4), col(5)
+            pair_obj = np.array([oidx[groups[r[0]]["obj_id"]] for r in pair_rows], np.int32)
+            pair_diam = torch.as_tensor(np.array([diam[groups[r[0]]["obj_id"]] for r in pair_rows], np.float32),
+                                        device=device)
+            done = stages.mark("vsd")
+            counts, errs = vsd(depth_test, K, fi, rdepth, rboxes, ei, rdepth, rboxes, gi_, pair_diam, delta, taus)
+            if done is not None:
+                done.record()
+            done = stages.mark("mssd_mspd")
+            mssd, mspd = mssd_mspd(torch.as_tensor(pair_obj, device=device), vo.tolist(), vertices, so.tolist(), syms, K,
+                                   fi, poses[ei.long()].contiguous(), poses[gi_.long()].contiguous())
+            if done is not None:
+                done.record()
+            out["group"].append(rows[:, 0])
+            out["est"].append(rows[:, 1])
+            out["gt"].append(rows[:, 2])
+            out["vsd"].append(errs.cpu().numpy())
+            out["vsd_counts"].append(counts.cpu().numpy())
+            out["mssd"].append(mssd.cpu().numpy())
+            out["mspd"].append(mspd.cpu().numpy())
+    if stage_ms is not None:
+        stage_ms.update(stages.totals())
+    if not out["group"]:
+        return dict(group=np.zeros(0, np.int64), est=np.zeros(0, np.int64), gt=np.zeros(0, np.int64),
+                    vsd=np.zeros((0, len(taus)), np.float32), vsd_counts=np.zeros((0, 2 + len(taus)), np.int32),
+                    mssd=np.zeros(0, np.float32), mspd=np.zeros(0, np.float32))
+    return {k: np.concatenate(v) for k, v in out.items()}
+
+
+def error_groups(setup, errors):
+    """Per target: the pairs' errors as [n_est, n_gt] tables in descending score order (the input of `recalls`)."""
+    groups = setup["groups"]
+    n_tau = errors["vsd"].shape[1]
+    out = []
+    for g in groups:
+        ne, ng = len(g["est"]), len(g["gt"])
+        out.append(dict(vsd=np.full((ne, ng, n_tau), np.inf), mssd=np.full((ne, ng), np.inf),
+                        mspd=np.full((ne, ng), np.inf), valid=g["valid"],
+                        diameter=setup["info"][g["obj_id"]]["diameter"]))
+    pos = [({e: i for i, e in enumerate(g["est"])}, {k: i for i, k in enumerate(g["gt"])}) for g in groups]
+    for p in range(len(errors["group"])):
+        gi = int(errors["group"][p])
+        a, b = pos[gi][0][int(errors["est"][p])], pos[gi][1][int(errors["gt"][p])]
+        out[gi]["vsd"][a, b] = errors["vsd"][p]
+        out[gi]["mssd"][a, b] = errors["mssd"][p]
+        out[gi]["mspd"][a, b] = errors["mspd"][p]
+    return out
+
+
+def average_time_per_image(results):
+    """Mean over the images with estimates of their csv `time` (the mean of the image's estimates), or -1 when an image
+    has none (time < 0) or there are no estimates."""
+    per = {}
+    for r in results:
+        per.setdefault((r["scene_id"], r["im_id"]), []).append(float(r.get("time", -1)))
+    if not per or any(min(t) < 0 for t in per.values()):
+        return -1.0
+    return float(np.mean([np.mean(t) for t in per.values()]))
+
+
+@torch.no_grad()
+def evaluate(results, dataset_dir, split="test", out_dir=None, device="cuda", delta=None, taus=TAUS,
+             theta_vsd=THETA_VSD, theta_mssd=THETA_MSSD, theta_mspd=THETA_MSPD,
+             targets_name="test_targets_bop19.json", stage_ms=None):
+    """BOP 2019 evaluation of `results` (a csv path or a list of `load_bop_results` dicts) on a BOP dataset directory.
+    -> dict(ar, ar_vsd, ar_mssd, ar_mspd, recall_vsd [n_tau, n_theta], recall_mssd, recall_mspd, n_targets,
+    average_time_per_image, errors (per pair, see `compute_errors`)); with `out_dir`, also writes
+    out_dir/scores_bop19.json with the keys the reference's eval_bop.py reads."""
+    setup = prepare(results, dataset_dir, split, targets_name)
+    errors = compute_errors(setup, device, delta, taus, stage_ms=stage_ms)
+    H_W = None
+    if setup["images"]:
+        s, im = setup["images"][0]
+        H_W = load_depth(dataset_dir, split, s, im, setup["scenes"][s]["depth_scale"][im]).shape
+    r = (H_W[1] if H_W else 640) / 640.0
+    n_targets = int(sum(g["valid"].sum() for g in setup["groups"]))
+    rec = recalls(error_groups(setup, errors), n_targets, taus, theta_vsd, theta_mssd, theta_mspd, r)
+    ar_vsd, ar_mssd, ar_mspd = float(rec["vsd"].mean()), float(rec["mssd"].mean()), float(rec["mspd"].mean())
+    out = dict(ar=(ar_vsd + ar_mssd + ar_mspd) / 3.0, ar_vsd=ar_vsd, ar_mssd=ar_mssd, ar_mspd=ar_mspd,
+               recall_vsd=rec["vsd"], recall_mssd=rec["mssd"], recall_mspd=rec["mspd"], n_targets=n_targets,
+               average_time_per_image=average_time_per_image(setup["results"]), errors=errors)
+    if out_dir is not None:
+        os.makedirs(out_dir, exist_ok=True)
+        scores = {"bop19_average_recall": out["ar"], "bop19_average_recall_vsd": ar_vsd,
+                  "bop19_average_recall_mssd": ar_mssd, "bop19_average_recall_mspd": ar_mspd,
+                  "bop19_average_time_per_image": out["average_time_per_image"]}
+        with open(os.path.join(out_dir, "scores_bop19.json"), "w") as f:
+            json.dump(scores, f, indent=2)
+    return out
+
+
+def main(argv=None):
+    ap = argparse.ArgumentParser(description="BOP 2019 pose-error evaluation (VSD, MSSD, MSPD, AR) on the GPU")
+    ap.add_argument("--results", required=True, help="BOP results csv")
+    ap.add_argument("--dataset-dir", required=True)
+    ap.add_argument("--split", default="test")
+    ap.add_argument("--out", default=None, help="directory for scores_bop19.json (default: next to the csv)")
+    a = ap.parse_args(argv)
+    out_dir = a.out if a.out is not None else os.path.dirname(os.path.abspath(a.results))
+    res = evaluate(a.results, a.dataset_dir, a.split, out_dir=out_dir)
+    print(json.dumps({k: res[k] for k in ("ar", "ar_vsd", "ar_mssd", "ar_mspd", "n_targets",
+                                          "average_time_per_image")}))
+
+
+if __name__ == "__main__":
+    main()

@@ -1,0 +1,262 @@
+// Row f7: the BOP 2019 pose-error metrics on the GPU, in place of the external BOP toolkit's eval_bop19_pose.py that
+// the reference calls (src/scripts/eval_bop.py:16-38).  Definitions: VSD, Hodan et al., "BOP: Benchmark for 6D Object
+// Pose Estimation", ECCV 2018; MSSD and MSPD, Hodan et al., "BOP Challenge 2020 on 6D Object Localization".
+// The host side (gigapose_b200/bop_eval.py) pairs estimates with ground truths, renders both with gp_render_depth and
+// matches the errors into recalls.
+//
+// Contract (what tests/test_gpu_bop_eval.py pins against oracle/bop_port.py, bit for bit):
+//  gp_bop_vsd, one CTA per (estimate, ground truth) pair, walking the union of the two render boxes (clipped to the
+//  image; no other pixel can be in either visibility mask).  Every operation below is one fp32 rounding
+//  (__fmul_rn / __fadd_rn / __fsub_rn / __fdiv_rn / __fsqrt_rn), no FMA contraction:
+//    distance of a depth z at pixel (u, v), K = [fx . cx; . fy cy] of the pair's frame (the skew is not used):
+//      X = ((u - cx) * z) / fx,  Y = ((v - cy) * z) / fy,  dist = sqrt((X * X + Y * Y) + z * z)   (0 for z = 0)
+//    with u, v the integer column and row (the rasteriser's pixel centre), for the test, estimate and GT depths;
+//    visib_gt  = dist_gt > 0 and ((dist_gt - dist_test) <= delta or dist_test == 0)
+//    visib_est = (dist_est > 0 and ((dist_est - dist_test) <= delta or dist_test == 0)) or (visib_gt and dist_est > 0)
+//    inter / union = pixels in both / either mask;  cost_t = pixels of inter with
+//      |dist_gt - dist_est| / diameter >= tau_t
+//    counts [n, 2 + n_tau] i32 = (inter, union, cost_0, ...);  e_t = float(cost_t + union - inter) / float(union),
+//    1 when union = 0 (an integer sum, then one rounding each to fp32, then one division).
+//  gp_bop_mssd_mspd, one CTA per (pair, chunk of kSymPerCta symmetry transforms) of the pair's object, threads over its
+//  vertices x:  s = S x (S = [S_R | S_t] of the transform),  g = P_gt s,  e = P_est x, each row ((A0 x + A1 y) + A2 z)
+//  + A3;  MSSD term = (dx * dx + dy * dy) + dz * dz with d = e - g;  MSPD term the same over the pixel differences of
+//  the two projections u = (K00 x + K01 y) / z + K02, v = (K11 y) / z + K12 (the rasteriser's projection).  The max
+//  over vertices is taken on the squared terms, then one sqrt, then the min over transforms with an atomicMin on the
+//  float bits: every value is >= 0 or NaN, so the unsigned bit order is the float order with NaN last, and both the
+//  max and the min are exact and independent of the schedule.
+#include "../../include/gigapose_b200.h"
+#include "gigapose_kernels.h"
+
+using gp::fail;
+
+namespace {
+
+constexpr int kThreads = 256;
+constexpr int kWarps = kThreads / 32;
+constexpr int kSymPerCta = 8;
+
+struct Taus {
+  float v[GP_BOP_MAX_TAU];
+};
+
+struct ObjectTables {                 // host offsets, by value: object o owns [off[o], off[o + 1])
+  int32_t vert_off[GP_BOP_MAX_OBJECTS + 1];
+  int32_t sym_off[GP_BOP_MAX_OBJECTS + 1];
+};
+
+__device__ __forceinline__ float distance(float z, int u, int v, float fx, float fy, float cx, float cy) {
+  const float X = __fdiv_rn(__fmul_rn(__fsub_rn((float)u, cx), z), fx);
+  const float Y = __fdiv_rn(__fmul_rn(__fsub_rn((float)v, cy), z), fy);
+  return __fsqrt_rn(__fadd_rn(__fadd_rn(__fmul_rn(X, X), __fmul_rn(Y, Y)), __fmul_rn(z, z)));
+}
+
+__device__ __forceinline__ bool visible(float d_model, float d_test, float delta) {
+  return d_model > 0.f && (__fsub_rn(d_model, d_test) <= delta || d_test == 0.f);
+}
+
+__global__ void __launch_bounds__(kThreads)
+vsd_kernel(int n_frames, int H, int W, const float* __restrict__ depth_test, const float* __restrict__ Kmat,
+           const int32_t* __restrict__ frame_idx, int n_est, const float* __restrict__ est_depth,
+           const long long* __restrict__ est_boxes, const int32_t* __restrict__ est_idx, int n_gt,
+           const float* __restrict__ gt_depth, const long long* __restrict__ gt_boxes,
+           const int32_t* __restrict__ gt_idx, const float* __restrict__ diameter, float delta, int n_tau, Taus taus,
+           int32_t* __restrict__ counts, float* __restrict__ errors) {
+  __shared__ int red[kWarps][2 + GP_BOP_MAX_TAU];
+  const int pair = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int f = frame_idx[pair], ie = est_idx[pair], ig = gt_idx[pair];
+  const int ncol = 2 + n_tau;
+  if (f < 0 || f >= n_frames || ie < 0 || ie >= n_est || ig < 0 || ig >= n_gt) {
+    for (int c = tid; c < ncol; c += kThreads) counts[(size_t)pair * ncol + c] = -1;
+    for (int c = tid; c < n_tau; c += kThreads) errors[(size_t)pair * n_tau + c] = __int_as_float(0x7fffffff);
+    return;
+  }
+  const float* K = Kmat + 9 * (size_t)f;
+  const float fx = K[0], cx = K[2], fy = K[4], cy = K[5];
+  const float diam = diameter[pair];
+  const long long* be = est_boxes + 4 * (size_t)ie;
+  const long long* bg = gt_boxes + 4 * (size_t)ig;
+  const int x0 = (int)max(min(be[0], bg[0]), 0ll), y0 = (int)max(min(be[1], bg[1]), 0ll);
+  const int x1 = (int)min(max(be[2], bg[2]), (long long)W), y1 = (int)min(max(be[3], bg[3]), (long long)H);
+  const size_t plane = (size_t)H * W;
+  const float* dt = depth_test + f * plane;
+  const float* de = est_depth + ie * plane;
+  const float* dg = gt_depth + ig * plane;
+  int cnt[2 + GP_BOP_MAX_TAU];
+#pragma unroll
+  for (int c = 0; c < 2 + GP_BOP_MAX_TAU; ++c) cnt[c] = 0;
+  const int bw = max(x1 - x0, 0), n = bw * max(y1 - y0, 0);
+  for (int p = tid; p < n; p += kThreads) {
+    const int v = y0 + p / bw, u = x0 + p % bw;
+    const size_t i = (size_t)v * W + u;
+    const float d_test = distance(dt[i], u, v, fx, fy, cx, cy);
+    const float d_gt = distance(dg[i], u, v, fx, fy, cx, cy);
+    const float d_est = distance(de[i], u, v, fx, fy, cx, cy);
+    const bool vg = visible(d_gt, d_test, delta);
+    const bool ve = visible(d_est, d_test, delta) || (vg && d_est > 0.f);
+    if (vg && ve) {
+      ++cnt[0];
+      const float c = __fdiv_rn(fabsf(__fsub_rn(d_gt, d_est)), diam);
+#pragma unroll
+      for (int t = 0; t < GP_BOP_MAX_TAU; ++t)
+        if (t < n_tau && c >= taus.v[t]) ++cnt[2 + t];
+    }
+    if (vg || ve) ++cnt[1];
+  }
+#pragma unroll
+  for (int c = 0; c < 2 + GP_BOP_MAX_TAU; ++c) {
+    const int s = __reduce_add_sync(0xffffffffu, cnt[c]);
+    if (lane == 0 && c < ncol) red[warp][c] = s;
+  }
+  __syncthreads();
+  if (tid < ncol) {
+    int s = 0;
+    for (int w = 0; w < kWarps; ++w) s += red[w][tid];
+    counts[(size_t)pair * ncol + tid] = s;
+    red[0][tid] = s;                    // column tid is read by no other thread before the barrier
+  }
+  __syncthreads();
+  if (tid < n_tau) {
+    const int inter = red[0][0], uni = red[0][1];
+    errors[(size_t)pair * n_tau + tid] =
+        uni == 0 ? 1.f : __fdiv_rn((float)(red[0][2 + tid] + uni - inter), (float)uni);
+  }
+}
+
+// ((A0 x + A1 y) + A2 z) + A3 for the three rows of a row-major [3,4] (or the top of a [4,4]) matrix
+__device__ __forceinline__ void affine(const float* A, float x, float y, float z, float o[3]) {
+#pragma unroll
+  for (int r = 0; r < 3; ++r)
+    o[r] = __fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(A[4 * r], x), __fmul_rn(A[4 * r + 1], y)), __fmul_rn(A[4 * r + 2], z)),
+                     A[4 * r + 3]);
+}
+
+__device__ __forceinline__ void project(const float* K, const float p[3], float& u, float& v) {
+  u = __fadd_rn(__fdiv_rn(__fadd_rn(__fmul_rn(K[0], p[0]), __fmul_rn(K[1], p[1])), p[2]), K[2]);
+  v = __fadd_rn(__fdiv_rn(__fmul_rn(K[4], p[1]), p[2]), K[5]);
+}
+
+__device__ __forceinline__ float sq3(float a, float b, float c) {
+  return __fadd_rn(__fadd_rn(__fmul_rn(a, a), __fmul_rn(b, b)), __fmul_rn(c, c));
+}
+
+__global__ void __launch_bounds__(kThreads)
+mssd_mspd_kernel(int n_objects, const int32_t* __restrict__ obj_idx, ObjectTables tab, const float* __restrict__ vertices,
+                 const float* __restrict__ syms, int n_frames, const float* __restrict__ Kmat,
+                 const int32_t* __restrict__ frame_idx, const float* __restrict__ pose_est,
+                 const float* __restrict__ pose_gt, float* __restrict__ mssd, float* __restrict__ mspd) {
+  __shared__ float sS[kSymPerCta][16], sPe[16], sPg[16], sK[9];
+  __shared__ unsigned red[kWarps][2 * kSymPerCta];
+  const int pair = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int o = obj_idx[pair], f = frame_idx[pair];
+  if (o < 0 || o >= n_objects || f < 0 || f >= n_frames) return;    // outputs keep their all-ones (NaN) bits
+  const int s0 = tab.sym_off[o] + blockIdx.y * kSymPerCta;
+  const int ns = min(tab.sym_off[o + 1] - s0, kSymPerCta);
+  if (ns <= 0) return;
+  for (int i = tid; i < ns * 16; i += kThreads) sS[i / 16][i % 16] = syms[16 * (size_t)s0 + i];
+  if (tid < 16) { sPe[tid] = pose_est[16 * (size_t)pair + tid]; sPg[tid] = pose_gt[16 * (size_t)pair + tid]; }
+  if (tid < 9) sK[tid] = Kmat[9 * (size_t)f + tid];
+  __syncthreads();
+  unsigned md[kSymPerCta], mp[kSymPerCta];
+#pragma unroll
+  for (int s = 0; s < kSymPerCta; ++s) md[s] = mp[s] = 0u;
+  const int v0 = tab.vert_off[o], v1 = tab.vert_off[o + 1];
+  for (int i = v0 + tid; i < v1; i += kThreads) {
+    const float x = vertices[3 * (size_t)i], y = vertices[3 * (size_t)i + 1], z = vertices[3 * (size_t)i + 2];
+    float e[3], ue, ve;
+    affine(sPe, x, y, z, e);
+    project(sK, e, ue, ve);
+#pragma unroll
+    for (int s = 0; s < kSymPerCta; ++s) {
+      if (s >= ns) break;
+      float sx[3], g[3], ug, vg;
+      affine(sS[s], x, y, z, sx);
+      affine(sPg, sx[0], sx[1], sx[2], g);
+      project(sK, g, ug, vg);
+      const float d = sq3(__fsub_rn(e[0], g[0]), __fsub_rn(e[1], g[1]), __fsub_rn(e[2], g[2]));
+      const float du = __fsub_rn(ue, ug), dv = __fsub_rn(ve, vg);
+      const float p = __fadd_rn(__fmul_rn(du, du), __fmul_rn(dv, dv));
+      md[s] = max(md[s], __float_as_uint(d));
+      mp[s] = max(mp[s], __float_as_uint(p));
+    }
+  }
+#pragma unroll
+  for (int s = 0; s < kSymPerCta; ++s) {
+    const unsigned a = __reduce_max_sync(0xffffffffu, md[s]), b = __reduce_max_sync(0xffffffffu, mp[s]);
+    if (lane == 0) { red[warp][s] = a; red[warp][kSymPerCta + s] = b; }
+  }
+  __syncthreads();
+  if (tid < 2) {
+    unsigned best = 0xffffffffu;
+    for (int s = 0; s < ns; ++s) {
+      unsigned m = 0u;
+      for (int w = 0; w < kWarps; ++w) m = max(m, red[w][tid * kSymPerCta + s]);
+      best = min(best, __float_as_uint(__fsqrt_rn(__uint_as_float(m))));
+    }
+    atomicMin(reinterpret_cast<unsigned*>(tid == 0 ? mssd : mspd) + pair, best);
+  }
+}
+
+constexpr int kMaxSide = 8192;
+
+}  // namespace
+
+extern "C" int gp_bop_vsd(int n_pairs, int n_frames, int height, int width, const float* depth_test, const float* K,
+                          const int32_t* frame_idx, int n_est, const float* est_depth, const int64_t* est_boxes,
+                          const int32_t* est_idx, int n_gt, const float* gt_depth, const int64_t* gt_boxes,
+                          const int32_t* gt_idx, const float* diameter, float delta, int n_tau, const float* tau,
+                          int32_t* counts, float* errors, void* stream) {
+  if (n_pairs < 1) return fail(GP_ERR_INVALID, "n_pairs %d must be >= 1", n_pairs);
+  if (n_frames < 1 || n_est < 1 || n_gt < 1)
+    return fail(GP_ERR_INVALID, "n_frames %d, n_est %d, n_gt %d must be >= 1", n_frames, n_est, n_gt);
+  if (height < 1 || width < 1 || height > kMaxSide || width > kMaxSide)
+    return fail(GP_ERR_INVALID, "image size %d x %d outside [1, %d]", height, width, kMaxSide);
+  if (n_tau < 1 || n_tau > GP_BOP_MAX_TAU) return fail(GP_ERR_INVALID, "n_tau %d outside [1, %d]", n_tau, GP_BOP_MAX_TAU);
+  if (!(delta > 0.f) || !isfinite(delta)) return fail(GP_ERR_INVALID, "delta must be positive and finite");
+  if (!tau) return fail(GP_ERR_INVALID, "null tau");
+  Taus taus;
+  for (int t = 0; t < n_tau; ++t) {
+    if (!(tau[t] > 0.f) || !isfinite(tau[t])) return fail(GP_ERR_INVALID, "tau[%d] must be positive and finite", t);
+    taus.v[t] = tau[t];
+  }
+  for (int t = n_tau; t < GP_BOP_MAX_TAU; ++t) taus.v[t] = 0.f;
+  if (!depth_test || !K || !frame_idx || !est_depth || !est_boxes || !est_idx || !gt_depth || !gt_boxes || !gt_idx ||
+      !diameter || !counts || !errors)
+    return fail(GP_ERR_INVALID, "null argument");
+  GP_CUDA(gp::launch_ex(vsd_kernel, n_pairs, kThreads, 0, static_cast<cudaStream_t>(stream), 1, false, n_frames, height,
+                        width, depth_test, K, frame_idx, n_est, est_depth, reinterpret_cast<const long long*>(est_boxes),
+                        est_idx, n_gt, gt_depth, reinterpret_cast<const long long*>(gt_boxes), gt_idx, diameter, delta,
+                        n_tau, taus, counts, errors));
+  return GP_OK;
+}
+
+extern "C" int gp_bop_mssd_mspd(int n_pairs, int n_objects, const int32_t* obj_idx, const int32_t* vertex_offsets,
+                                const float* vertices, const int32_t* sym_offsets, const float* syms, int n_frames,
+                                const float* K, const int32_t* frame_idx, const float* pose_est, const float* pose_gt,
+                                float* mssd, float* mspd, void* stream) {
+  if (n_pairs < 1) return fail(GP_ERR_INVALID, "n_pairs %d must be >= 1", n_pairs);
+  if (n_objects < 1 || n_objects > GP_BOP_MAX_OBJECTS)
+    return fail(GP_ERR_INVALID, "n_objects %d outside [1, %d]", n_objects, GP_BOP_MAX_OBJECTS);
+  if (n_frames < 1) return fail(GP_ERR_INVALID, "n_frames %d must be >= 1", n_frames);
+  if (!vertex_offsets || !sym_offsets) return fail(GP_ERR_INVALID, "null offsets");
+  ObjectTables tab;
+  int max_syms = 0;
+  for (int o = 0; o <= n_objects; ++o) {
+    tab.vert_off[o] = vertex_offsets[o];
+    tab.sym_off[o] = sym_offsets[o];
+    if (o == 0 ? vertex_offsets[0] != 0 || sym_offsets[0] != 0
+               : vertex_offsets[o] <= vertex_offsets[o - 1] || sym_offsets[o] <= sym_offsets[o - 1])
+      return fail(GP_ERR_INVALID, "bad offsets at object %d: they must start at 0 and increase strictly "
+                  "(every object has a vertex and a transform)", o);
+    if (o > 0) max_syms = max(max_syms, sym_offsets[o] - sym_offsets[o - 1]);
+  }
+  for (int o = n_objects + 1; o <= GP_BOP_MAX_OBJECTS; ++o) tab.vert_off[o] = tab.sym_off[o] = 0;
+  if (!obj_idx || !vertices || !syms || !K || !frame_idx || !pose_est || !pose_gt || !mssd || !mspd)
+    return fail(GP_ERR_INVALID, "null argument");
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  GP_CUDA(cudaMemsetAsync(mssd, 0xFF, (size_t)n_pairs * sizeof(float), st));
+  GP_CUDA(cudaMemsetAsync(mspd, 0xFF, (size_t)n_pairs * sizeof(float), st));
+  GP_CUDA(gp::launch_ex(mssd_mspd_kernel, dim3(n_pairs, (max_syms + kSymPerCta - 1) / kSymPerCta), kThreads, 0, st, 1,
+                        false, n_objects, obj_idx, tab, vertices, syms, n_frames, K, frame_idx, pose_est, pose_gt, mssd,
+                        mspd));
+  return GP_OK;
+}

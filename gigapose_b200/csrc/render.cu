@@ -25,6 +25,10 @@
 //  - Resolve, one thread per pixel: RGB = round(255 * mean of the 4 samples (background = 0)) / 255, the 8-bit
 //    framebuffer + PNG round trip; alpha = 1 if any sample is covered; depth = the smallest covered sample z, else 0.
 //  - Boxes: [x0, y0, x1, y1) of alpha > 0 with exclusive max (PIL getbbox), (0, 0, W, H) for an empty view.
+//  - Depth only (gp_render_depth, the depth maps of the BOP pose-error metrics): the same raster with ONE sample per
+//    pixel at offset (0, 0), i.e. at the pixel centre as the BOP renderers take it; depth = that sample's z (0 =
+//    background), boxes of depth > 0; no shading and no RGBA.  The sample count is a template parameter of the raster
+//    and resolve code, so both entry points share every line of the arithmetic above.
 //
 // Layout: one thread per (view, face) sets the triangle up and rasterises it alone when its pixel bounding box is at
 // most kSmallPixels; larger triangles are queued in shared memory and rasterised by the whole CTA, so neither a mesh
@@ -41,9 +45,14 @@ constexpr int kSmallPixels = 32;
 constexpr float kGuardPx = 4194304.f;                    // 2^22 px: snapped |coordinate| < 2^30
 constexpr unsigned long long kEmpty = ~0ull;
 
-// sample offsets in 1/256 px
-__device__ __forceinline__ int sample_dx(int s) { return s == 0 ? -32 : s == 1 ? 96 : s == 2 ? -96 : 32; }
-__device__ __forceinline__ int sample_dy(int s) { return s == 0 ? -96 : s == 1 ? -32 : s == 2 ? 32 : 96; }
+// sample offsets in 1/256 px: the rotated grid of 4x MSAA, or the pixel centre for one sample
+template <int NS>
+__device__ __forceinline__ int sample_dx(int s) { return NS == 1 ? 0 : s == 0 ? -32 : s == 1 ? 96 : s == 2 ? -96 : 32; }
+template <int NS>
+__device__ __forceinline__ int sample_dy(int s) { return NS == 1 ? 0 : s == 0 ? -96 : s == 1 ? -32 : s == 2 ? 32 : 96; }
+// largest |offset| of a sample from its pixel centre, 1/256 px
+template <int NS>
+constexpr int sample_reach() { return NS == 1 ? 0 : 96; }
 
 struct Tri {
   int x[3], y[3];          // snapped screen positions (1/256 px), ordered so that the doubled area is positive
@@ -127,13 +136,14 @@ __device__ __forceinline__ float sample_depth(const float b[3]) {
   return __frcp_rn(__fadd_rn(__fadd_rn(b[0], b[1]), b[2]));
 }
 
+template <int NS>
 __device__ __forceinline__ void raster_pixel(const Tri& t, int face, int px, int py, int W,
                                              unsigned long long* __restrict__ keys) {
-  unsigned long long* k = keys + ((size_t)py * W + px) * 4;
+  unsigned long long* k = keys + ((size_t)py * W + px) * NS;
 #pragma unroll
-  for (int s = 0; s < 4; ++s) {
+  for (int s = 0; s < NS; ++s) {
     float b[3];
-    if (!sample_weights(t, px * 256 + sample_dx(s), py * 256 + sample_dy(s), b)) continue;
+    if (!sample_weights(t, px * 256 + sample_dx<NS>(s), py * 256 + sample_dy<NS>(s), b)) continue;
     const unsigned long long key =
         ((unsigned long long)__float_as_uint(sample_depth(b)) << 32) | (unsigned long long)(unsigned)face;
     atomicMin(k + s, key);
@@ -142,6 +152,7 @@ __device__ __forceinline__ void raster_pixel(const Tri& t, int face, int px, int
 
 __device__ __forceinline__ int floor_div256(int a) { return a >> 8; }   // arithmetic shift == floor division
 
+template <int NS>
 __global__ void __launch_bounds__(kThreads)
 raster_kernel(int H, int W, int nv, const float* __restrict__ V, int nf, const int* __restrict__ faces,
               const float* __restrict__ poses, const float* __restrict__ Kmat, float z_near,
@@ -155,19 +166,20 @@ raster_kernel(int H, int W, int nv, const float* __restrict__ V, int nf, const i
   if (tid < 6) sK[tid] = Kmat[tid];
   if (tid == 0) nbig = 0;
   __syncthreads();
-  keys += (size_t)view * H * W * 4;
+  keys += (size_t)view * H * W * NS;
   const int f = blockIdx.x * kThreads + tid;
   Tri t;
   if (f < nf && setup_triangle(f, nv, V, faces, sP, sK, z_near, t)) {
     const int xmin = min(min(t.x[0], t.x[1]), t.x[2]), xmax = max(max(t.x[0], t.x[1]), t.x[2]);
     const int ymin = min(min(t.y[0], t.y[1]), t.y[2]), ymax = max(max(t.y[0], t.y[1]), t.y[2]);
-    // pixel i holds samples at 256 i + [-96, 96]
-    const int px0 = max(-floor_div256(96 - xmin), 0), px1 = min(floor_div256(xmax + 96), W - 1);
-    const int py0 = max(-floor_div256(96 - ymin), 0), py1 = min(floor_div256(ymax + 96), H - 1);
+    // pixel i holds samples at 256 i + [-reach, reach]
+    constexpr int R = sample_reach<NS>();
+    const int px0 = max(-floor_div256(R - xmin), 0), px1 = min(floor_div256(xmax + R), W - 1);
+    const int py0 = max(-floor_div256(R - ymin), 0), py1 = min(floor_div256(ymax + R), H - 1);
     if (px0 <= px1 && py0 <= py1) {
       if ((long long)(px1 - px0 + 1) * (py1 - py0 + 1) <= kSmallPixels) {
         for (int py = py0; py <= py1; ++py)
-          for (int px = px0; px <= px1; ++px) raster_pixel(t, f, px, py, W, keys);
+          for (int px = px0; px <= px1; ++px) raster_pixel<NS>(t, f, px, py, W, keys);
       } else {
         const int slot = atomicAdd(&nbig, 1);                // queue order is irrelevant: atomicMin decides
         big[slot] = t;
@@ -181,7 +193,7 @@ raster_kernel(int H, int W, int nv, const float* __restrict__ V, int nf, const i
     const int bw = big_box[i][2], n = bw * big_box[i][3];
     for (int p = tid; p < n; p += kThreads) {
       const int py = p / bw;
-      raster_pixel(big[i], big_face[i], big_box[i][0] + p - py * bw, big_box[i][1] + py, W, keys);
+      raster_pixel<NS>(big[i], big_face[i], big_box[i][0] + p - py * bw, big_box[i][1] + py, W, keys);
     }
   }
 }
@@ -223,6 +235,8 @@ __device__ __forceinline__ float interpolate(const float b[3], float z, float a0
   return __fmul_rn(__fadd_rn(__fadd_rn(__fmul_rn(b[0], a0), __fmul_rn(b[1], a1)), __fmul_rn(b[2], a2)), z);
 }
 
+// kShade = false: depth only (rgba and the shading inputs are not read)
+template <int NS, bool kShade>
 __global__ void __launch_bounds__(kThreads)
 resolve_kernel(int H, int W, int nv, const float* __restrict__ V, const int* __restrict__ faces,
                const float* __restrict__ vcolor, const float* __restrict__ face_uv, const float* __restrict__ tex,
@@ -238,21 +252,22 @@ resolve_kernel(int H, int W, int nv, const float* __restrict__ V, const int* __r
   const int pix = blockIdx.x * kThreads + tid;
   if (pix >= H * W) return;
   const int py = pix / W, px = pix - py * W;
-  const unsigned long long* k = keys + ((size_t)view * H * W + pix) * 4;
+  const unsigned long long* k = keys + ((size_t)view * H * W + pix) * NS;
   float sum[3] = {0.f, 0.f, 0.f};
   float zmin = 0.f;
   bool covered = false;
-  for (int s = 0; s < 4; ++s) {
+  for (int s = 0; s < NS; ++s) {
     const unsigned long long key = k[s];
     if (key == kEmpty) continue;                                       // background sample: adds 0
     const int f = (int)(unsigned)(key & 0xffffffffull);
     const float zs = __uint_as_float((unsigned)(key >> 32));
     zmin = covered ? fminf(zmin, zs) : zs;
     covered = true;
+    if (!kShade) continue;
     Tri t;
     float b[3], c[3];
     setup_triangle(f, nv, V, faces, sP, sK, z_near, t);               // same arithmetic as the raster pass
-    sample_weights(t, px * 256 + sample_dx(s), py * 256 + sample_dy(s), b);
+    sample_weights(t, px * 256 + sample_dx<NS>(s), py * 256 + sample_dy<NS>(s), b);
     const float z = sample_depth(b);
     if (tex) {
       const float* uv = face_uv + 6 * (size_t)f;
@@ -271,23 +286,26 @@ resolve_kernel(int H, int W, int nv, const float* __restrict__ V, const int* __r
     for (int ch = 0; ch < 3; ++ch) sum[ch] = __fadd_rn(sum[ch], c[ch]);
   }
   const size_t plane = (size_t)H * W;
-  float* out = rgba + (size_t)view * 4 * plane + pix;
-  for (int ch = 0; ch < 3; ++ch) {
-    const float q = fminf(fmaxf(rintf(__fmul_rn(__fmul_rn(sum[ch], 0.25f), 255.f)), 0.f), 255.f);
-    out[ch * plane] = __fdiv_rn(q, 255.f);
+  if (kShade) {
+    static_assert(!kShade || NS == 4, "the shaded resolve averages 4 samples");
+    float* out = rgba + (size_t)view * 4 * plane + pix;
+    for (int ch = 0; ch < 3; ++ch) {
+      const float q = fminf(fmaxf(rintf(__fmul_rn(__fmul_rn(sum[ch], 0.25f), 255.f)), 0.f), 255.f);
+      out[ch * plane] = __fdiv_rn(q, 255.f);
+    }
+    out[3 * plane] = covered ? 1.f : 0.f;
   }
-  out[3 * plane] = covered ? 1.f : 0.f;
   if (depth) depth[(size_t)view * plane + pix] = covered ? zmin : 0.f;
 }
 
-// one CTA per view: [x0, y0, x1, y1) of alpha > 0
+// one CTA per view: [x0, y0, x1, y1) of the pixels > 0 of the plane at mask + view * view_stride (alpha, or depth)
 __global__ void __launch_bounds__(kThreads)
-boxes_kernel(int H, int W, const float* __restrict__ rgba, long long* __restrict__ boxes) {
+boxes_kernel(int H, int W, const float* __restrict__ mask, size_t view_stride, long long* __restrict__ boxes) {
   __shared__ int b[4];
   const int view = blockIdx.x;
   if (threadIdx.x == 0) { b[0] = W; b[1] = H; b[2] = -1; b[3] = -1; }
   __syncthreads();
-  const float* alpha = rgba + ((size_t)view * 4 + 3) * H * W;
+  const float* alpha = mask + view * view_stride;
   int x0 = W, y0 = H, x1 = -1, y1 = -1;
   for (int p = threadIdx.x; p < H * W; p += kThreads) {
     if (alpha[p] > 0.f) {
@@ -344,12 +362,36 @@ extern "C" int gp_render_templates(int n_views, int height, int width, int num_v
   const size_t key_bytes = (size_t)n_views * height * width * 4 * sizeof(unsigned long long);
   GP_CUDA(cudaMemsetAsync(keys, 0xFF, key_bytes, st));
   if (num_faces > 0)
-    GP_CUDA(gp::launch_ex(raster_kernel, dim3((num_faces + kThreads - 1) / kThreads, n_views), kThreads, 0, st, 1, false,
+    GP_CUDA(gp::launch_ex(raster_kernel<4>, dim3((num_faces + kThreads - 1) / kThreads, n_views), kThreads, 0, st, 1, false,
                           height, width, num_vertices, vertices, num_faces, faces, poses, K, z_near, keys));
-  GP_CUDA(gp::launch_ex(resolve_kernel, dim3((height * width + kThreads - 1) / kThreads, n_views), kThreads, 0, st, 1, false,
+  GP_CUDA(gp::launch_ex(resolve_kernel<4, true>, dim3((height * width + kThreads - 1) / kThreads, n_views), kThreads, 0, st, 1, false,
                         height, width, num_vertices, vertices, faces, vertex_color, face_uv, texture, tex_h, tex_w,
                         constant_color, poses, K, z_near, keys, rgba, depth));
-  GP_CUDA(gp::launch_ex(boxes_kernel, n_views, kThreads, 0, st, 1, false, height, width, rgba,
+  GP_CUDA(gp::launch_ex(boxes_kernel, n_views, kThreads, 0, st, 1, false, height, width, rgba + 3 * (size_t)height * width,
+                        (size_t)4 * height * width, reinterpret_cast<long long*>(boxes)));
+  return GP_OK;
+}
+
+extern "C" int gp_render_depth(int n_views, int height, int width, int num_vertices, const float* vertices,
+                               int num_faces, const int32_t* faces, const float* poses, const float* K, float z_near,
+                               void* workspace, float* depth, int64_t* boxes, void* stream) {
+  if (const int rc = check_sizes(n_views, height, width)) return rc;
+  if (num_vertices < 0 || num_faces < 0) return fail(GP_ERR_INVALID, "negative mesh size");
+  if (!(z_near > 0.f) || !isfinite(z_near)) return fail(GP_ERR_INVALID, "z_near must be positive and finite");
+  if (!poses || !K || !workspace || !depth || !boxes) return fail(GP_ERR_INVALID, "null argument");
+  if (num_faces > 0 && (!vertices || !faces || num_vertices < 1))
+    return fail(GP_ERR_INVALID, "null argument (mesh)");
+  if (n_views == 0) return GP_OK;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  auto* keys = static_cast<unsigned long long*>(workspace);
+  GP_CUDA(cudaMemsetAsync(keys, 0xFF, (size_t)n_views * height * width * sizeof(unsigned long long), st));
+  if (num_faces > 0)
+    GP_CUDA(gp::launch_ex(raster_kernel<1>, dim3((num_faces + kThreads - 1) / kThreads, n_views), kThreads, 0, st, 1, false,
+                          height, width, num_vertices, vertices, num_faces, faces, poses, K, z_near, keys));
+  GP_CUDA(gp::launch_ex(resolve_kernel<1, false>, dim3((height * width + kThreads - 1) / kThreads, n_views), kThreads, 0, st,
+                        1, false, height, width, num_vertices, vertices, faces, nullptr, nullptr, nullptr, 0, 0, nullptr,
+                        poses, K, z_near, keys, nullptr, depth));
+  GP_CUDA(gp::launch_ex(boxes_kernel, n_views, kThreads, 0, st, 1, false, height, width, depth, (size_t)height * width,
                         reinterpret_cast<long long*>(boxes)));
   return GP_OK;
 }

@@ -289,6 +289,44 @@ int gp_render_templates(int n_views, int height, int width, int num_vertices, co
                         const int32_t* faces, const float* vertex_color, const float* face_uv, const float* texture,
                         int tex_h, int tex_w, const float* constant_color, const float* poses, const float* K,
                         float z_near, void* workspace, float* rgba, float* depth, int64_t* boxes, void* stream);
+/* Depth-only renders for the pose-error metrics (row f7; the BOP toolkit's vispy depth renderer, which the reference
+ * reaches through eval_bop19_pose.py, src/scripts/eval_bop.py:16-38): the mesh, poses, K and z_near of
+ * gp_render_templates, rasterised with ONE sample per pixel at the pixel centre and no shading.  Outputs: depth f32
+ * [n,H,W] (0 = background), boxes i64 [n,4] of depth > 0 (xyxy, exclusive max; (0, 0, W, H) for an empty view).
+ * `workspace` holds n_views * H * W * 8 bytes (one u64 depth key per pixel). */
+int gp_render_depth(int n_views, int height, int width, int num_vertices, const float* vertices, int num_faces,
+                    const int32_t* faces, const float* poses, const float* K, float z_near, void* workspace, float* depth,
+                    int64_t* boxes, void* stream);
+
+/* --- row f7: BOP 2019 pose errors (the BOP toolkit's VSD / MSSD / MSPD that eval_bop19_pose.py computes for the
+ * reference, src/scripts/eval_bop.py:16-38).  The full contract, with the fp32 operation order, is the header comment
+ * of gigapose_b200/csrc/bop_eval.cu.  Needs no handle. -------------------------------------------------------------- */
+#define GP_BOP_MAX_TAU 16         /* VSD misalignment tolerances per call */
+#define GP_BOP_MAX_OBJECTS 256    /* objects per gp_bop_mssd_mspd call */
+/* VSD (step cost, normalised by the diameter, BOP 2019 visibility) of n_pairs (estimate, ground truth) pairs.
+ *   depth_test f32 [n_frames,H,W] measured depth in the model unit (0 = missing), K f32 [n_frames,3,3];
+ *   est_depth f32 [n_est,H,W] / est_boxes i64 [n_est,4] and gt_depth / gt_boxes likewise (gp_render_depth outputs);
+ *   per pair: frame_idx, est_idx, gt_idx i32 [n_pairs] (one render serves every pair it belongs to), diameter f32;
+ *   delta > 0 and tau (HOST f32 [n_tau], 1 <= n_tau <= GP_BOP_MAX_TAU, each > 0) in the diameter-normalised unit.
+ * Outputs: counts i32 [n_pairs, 2 + n_tau] = (inter, union, cost per tau), errors f32 [n_pairs, n_tau]
+ * ((cost + union - inter) / union, 1 for an empty union).  A pair with an index out of range gets counts -1 and
+ * errors NaN. */
+int gp_bop_vsd(int n_pairs, int n_frames, int height, int width, const float* depth_test, const float* K,
+               const int32_t* frame_idx, int n_est, const float* est_depth, const int64_t* est_boxes,
+               const int32_t* est_idx, int n_gt, const float* gt_depth, const int64_t* gt_boxes, const int32_t* gt_idx,
+               const float* diameter, float delta, int n_tau, const float* tau, int32_t* counts, float* errors,
+               void* stream);
+/* MSSD (model unit) and MSPD (px) of n_pairs pairs: min over the object's symmetry transforms S of max over its
+ * vertices x of |P_est x - P_gt S x|, and of the distance between the two points projected with the frame's K.
+ *   obj_idx i32 [n_pairs] (0-based), vertices f32 [sum V_o, 3] and syms f32 [sum S_o, 4, 4] concatenated per object,
+ *   with HOST offsets vertex_offsets / sym_offsets i32 [n_objects + 1] (0 first, strictly increasing: every object has
+ *   a vertex and a transform, the identity included); K f32 [n_frames,3,3], frame_idx i32 [n_pairs], pose_est /
+ *   pose_gt f32 [n_pairs,4,4] object -> camera.
+ * Outputs mssd, mspd f32 [n_pairs]; a pair whose object or frame index is out of range gets NaN. */
+int gp_bop_mssd_mspd(int n_pairs, int n_objects, const int32_t* obj_idx, const int32_t* vertex_offsets,
+                     const float* vertices, const int32_t* sym_offsets, const float* syms, int n_frames, const float* K,
+                     const int32_t* frame_idx, const float* pose_est, const float* pose_gt, float* mssd, float* mspd,
+                     void* stream);
 
 /* --- row f6: depth refinement of the coarse poses (MegaPose's ICPRefiner, src/megapose/inference/icp_refiner.py:134-287,
  * with a GPU point-to-plane ICP in place of OpenCV's ppf_match_3d_ICP).  The full contract is the header comment of
