@@ -20,6 +20,10 @@ PRECISION_BF16 = 1
 MAX_NUM_TEMPLATES = 12032      # GP_MAX_NUM_TEMPLATES: largest num_templates per handle
 BOP_MAX_TAU = 16               # GP_BOP_MAX_TAU
 BOP_MAX_OBJECTS = 256          # GP_BOP_MAX_OBJECTS
+BOP_MAX_GT_PER_GROUP = 1024    # GP_BOP_MAX_GT_PER_GROUP
+BOP_MAX_RECALL = 128           # GP_BOP_MAX_RECALL
+BOP_MATCH_GROUP_BYTES = 32     # GP_BOP_MATCH_GROUP_BYTES
+BOP_LABEL_FP, BOP_LABEL_TP, BOP_LABEL_IGNORED = 0, 1, 2          # GP_BOP_LABEL_*
 
 
 class GpConfig(C.Structure):
@@ -142,6 +146,12 @@ SYMBOLS = {
     "gp_bop_mssd_mspd": (C.c_int, [C.c_int, C.c_int, C.c_void_p, C.POINTER(C.c_int32), C.c_void_p, C.POINTER(C.c_int32),
                                    C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                    C.c_void_p, C.c_void_p]),
+    "gp_bop_match": (C.c_int, [C.c_int, C.c_int, C.c_int, C.POINTER(C.c_int32), C.POINTER(C.c_int32),
+                               C.POINTER(C.c_int32), C.POINTER(C.c_double), C.c_void_p, C.c_void_p, C.c_void_p,
+                               C.c_void_p, C.c_void_p, C.c_void_p]),
+    "gp_bop_average_precision": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_void_p, C.POINTER(C.c_int32), C.c_void_p,
+                                           C.POINTER(C.c_int32), C.c_int, C.POINTER(C.c_double), C.c_void_p,
+                                           C.c_void_p]),
     "gp_icp_query_sizes": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_size_t)]),
     "gp_icp_prepare_scene": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_float, C.c_void_p,
                                        C.c_void_p]),

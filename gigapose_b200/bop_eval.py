@@ -3,9 +3,15 @@ BOP toolkit's eval_bop19_pose.py that the reference shells out to (src/scripts/e
 
 Estimates and ground truths are rendered with `gp_render_depth` (one depth sample at each pixel centre), the per-pixel
 VSD counts and the symmetry-aware vertex distances run in csrc/bop_eval.cu (whose header comment states the fp32
-contract), and the matching into recalls runs here in numpy.  Usage:
+contract), and the matching into recalls runs here in numpy.
+
+Row f8 scores the BOP 2024 6D-detection task (`evaluate_detection`): MSSD and MSPD of every kept estimate against every
+ground truth of its object in its image, then the greedy matching with ignored ground truths and the COCO average
+precision, all on the device (gp_bop_mssd_mspd, gp_bop_match, gp_bop_average_precision).  No depth images are read.
+Usage:
 
     python -m gigapose_b200.bop_eval --results X.csv --dataset-dir D [--split test] [--out DIR]
+    python -m gigapose_b200.bop_eval --task detection --results X.csv --dataset-dir D [--split test] [--out DIR]
 """
 from __future__ import annotations
 
@@ -461,14 +467,240 @@ def evaluate(results, dataset_dir, split="test", out_dir=None, device="cuda", de
     return out
 
 
+# ---------------------------------------------------------------------------------------------------- BOP 2024 detection
+# Row f8: the 6D-detection task of BOP 2024 (the reference's `test_setting: detection`, scored with the toolkit's
+# eval_bop24_pose.py): every estimate competes, ground truths below VISIB_GT_MIN are ignored rather than missed, and the
+# score is COCO-style average precision over MSSD and MSPD.  The statement, with its operation order, is the header
+# comment of csrc/bop_eval.cu; the constants below are taken from it and are unverified against eval_bop24_pose.py.
+TARGETS_BOP24 = "test_targets_bop24.json"
+MAX_ESTIMATES_PER_IMAGE = 100   # highest scores kept per image (stable: csv order on ties)
+RECALL_THRESHOLDS = np.linspace(0.0, 1.0, 101)                   # COCO's 101 recall points
+MAX_PAIRS_PER_CALL = 1 << 18    # pairs per gp_bop_mssd_mspd call: ~140 B of poses, indices and errors each, ~37 MB
+
+
+def load_target_images(dataset_dir, name=TARGETS_BOP24):
+    """-> [(scene_id, im_id)] of a targets file, once each in order of first appearance.  Other keys (obj_id,
+    inst_count) are ignored, so both the BOP 2019 and the BOP 2024 target formats load."""
+    out = {}
+    for t in _json(os.path.join(dataset_dir, name)):
+        out.setdefault((int(t["scene_id"]), int(t["im_id"])), None)
+    return list(out)
+
+
+def image_width(dataset_dir, split, scene_id, im_id):
+    """Width in pixels, from the header of the image's file under depth/, rgb/ or gray/ (the first that has it)."""
+    import glob
+    from PIL import Image
+    d = os.path.join(dataset_dir, split, f"{scene_id:06d}")
+    for sub in ("depth", "rgb", "gray"):
+        found = sorted(glob.glob(os.path.join(glob.escape(os.path.join(d, sub)), f"{im_id:06d}.*")))
+        if found:
+            with Image.open(found[0]) as im:
+                return int(im.size[0])
+    raise BopEvalError(f"no image {im_id:06d} under {d}/depth, rgb or gray: the image width sets the MSPD threshold")
+
+
+def prepare_detection(results, dataset_dir, split="test", targets_name=TARGETS_BOP24,
+                      max_estimates_per_image=MAX_ESTIMATES_PER_IMAGE):
+    """Host side of the detection score: the target images, every ground truth in them (valid when visib_fract >=
+    VISIB_GT_MIN, ignored otherwise), the evaluated objects (those with a valid ground truth), and per image the
+    max_estimates_per_image highest-scoring estimates (stable sort: csv order on ties) of which those of evaluated
+    objects are kept.  -> dict with `images`, `objects`, `n_valid` {obj: valid ground truths}, and `groups`: one per
+    (image, evaluated object) with a kept estimate or a ground truth, dict(scene_id, im_id, obj_id, est (result indices
+    in descending score order), gt (instance indices in scene_gt), valid [n_gt] bool)."""
+    results = load_results(results)
+    images = load_target_images(dataset_dir, targets_name)
+    mdir = models_dir(dataset_dir)
+    info = load_models_info(mdir)
+    scenes = {}
+    n_valid = {}
+    for s, im in images:
+        if s not in scenes:
+            scenes[s] = load_scene(dataset_dir, split, s)
+        if im not in scenes[s]["gt"] or im not in scenes[s]["K"]:
+            raise BopEvalError(f"target image {s}/{im} is not in scene_gt.json / scene_camera.json")
+        for g, v in zip(scenes[s]["gt"][im], scenes[s]["visib"][im]):
+            if v >= VISIB_GT_MIN:
+                n_valid[g["obj_id"]] = n_valid.get(g["obj_id"], 0) + 1
+    objects = sorted(n_valid)
+    for o in objects:
+        if o not in info:
+            raise BopEvalError(f"object {o} of a ground truth is not in {mdir}/models_info.json")
+    by_image = {}
+    for i, res in enumerate(results):
+        by_image.setdefault((res["scene_id"], res["im_id"]), []).append(i)
+    groups = []
+    for s, im in images:
+        ests = sorted(by_image.get((s, im), []), key=lambda i: -results[i]["score"])[:max_estimates_per_image]
+        insts, visib = scenes[s]["gt"][im], scenes[s]["visib"][im]
+        for o in objects:
+            est = [i for i in ests if results[i]["obj_id"] == o]
+            gt = [k for k, g in enumerate(insts) if g["obj_id"] == o]
+            if est or gt:
+                groups.append(dict(scene_id=s, im_id=im, obj_id=o, est=est, gt=gt,
+                                   valid=np.array([visib[k] >= VISIB_GT_MIN for k in gt], bool)))
+    return dict(results=results, images=images, scenes=scenes, info=info, mdir=mdir, dataset_dir=dataset_dir,
+                split=split, objects=objects, n_valid=n_valid, groups=groups)
+
+
+def detection_pairs(setup):
+    """Every (kept estimate, ground truth) pair of each group, group after group, each group a row-major [n_est, n_gt]
+    block (the layout gp_bop_match reads).  -> dict of int64 arrays over the pairs: group, est (result index), gt
+    (instance index), frame (index in setup["images"])."""
+    frame = {key: f for f, key in enumerate(setup["images"])}
+    cols = dict(group=[], est=[], gt=[], frame=[])
+    for gi, g in enumerate(setup["groups"]):
+        ne, ng = len(g["est"]), len(g["gt"])
+        if ne and ng:
+            cols["group"].append(np.full(ne * ng, gi))
+            cols["est"].append(np.repeat(np.asarray(g["est"], np.int64), ng))
+            cols["gt"].append(np.tile(np.asarray(g["gt"], np.int64), ne))
+            cols["frame"].append(np.full(ne * ng, frame[(g["scene_id"], g["im_id"])]))
+    return {k: np.concatenate(v).astype(np.int64) if v else np.zeros(0, np.int64) for k, v in cols.items()}
+
+
+def _int32p(a):
+    return a.ctypes.data_as(C.POINTER(C.c_int32))
+
+
+@torch.no_grad()
+def evaluate_detection(results, dataset_dir, split="test", out_dir=None, device="cuda", theta_mssd=THETA_MSSD,
+                       theta_mspd=THETA_MSPD, targets_name=TARGETS_BOP24,
+                       max_estimates_per_image=MAX_ESTIMATES_PER_IMAGE, stage_ms=None):
+    """BOP 2024 6D-detection score of `results` (a csv path or a list of `load_bop_results` dicts) on a BOP dataset
+    directory; needs no depth images.  MSSD / MSPD of every pair (gp_bop_mssd_mspd, at most MAX_PAIRS_PER_CALL pairs
+    per call), the matching (gp_bop_match) and the AP (gp_bop_average_precision) run on the device in stream order.
+    -> dict(map, map_mssd, map_mspd, ap_mssd / ap_mspd [n_objects, n_theta], objects, average_time_per_image,
+    errors (per pair: group, est, gt, mssd, mspd), labels i8 [n_rows, 2, n_theta] (GP_BOP_LABEL_*), rows (result index
+    of each label row)); with `out_dir`, also writes out_dir/scores_bop24.json.  `stage_ms` (a dict) receives the
+    CUDA-event milliseconds of the stages mssd_mspd / match / ap."""
+    device = _lib.cuda_device(device, "BOP evaluation")
+    T = len(theta_mssd)
+    if len(theta_mspd) != T or not 1 <= T <= _lib.BOP_MAX_TAU:
+        raise BopEvalError(f"MSSD and MSPD need the same number of thresholds, between 1 and {_lib.BOP_MAX_TAU}")
+    setup = prepare_detection(results, dataset_dir, split, targets_name, max_estimates_per_image)
+    objects, groups, res, scenes, info = (setup[k] for k in ("objects", "groups", "results", "scenes", "info"))
+    if not objects:
+        raise BopEvalError(f"no target image has a ground truth with visib_fract >= {VISIB_GT_MIN}")
+    if len(objects) > _lib.BOP_MAX_OBJECTS:
+        raise BopEvalError(f"at most {_lib.BOP_MAX_OBJECTS} objects per evaluation, got {len(objects)}")
+    for g in groups:
+        if len(g["gt"]) > _lib.BOP_MAX_GT_PER_GROUP:
+            raise BopEvalError(f"image {g['scene_id']}/{g['im_id']} has {len(g['gt'])} instances of object "
+                               f"{g['obj_id']}, more than {_lib.BOP_MAX_GT_PER_GROUP}")
+    oidx = {o: i for i, o in enumerate(objects)}
+    s0, im0 = setup["images"][0]
+    r = image_width(dataset_dir, split, s0, im0) / 640.0
+    pairs = detection_pairs(setup)
+    n_pairs, n_obj = len(pairs["group"]), len(objects)
+    est_off = np.concatenate([[0], np.cumsum([len(g["est"]) for g in groups])]).astype(np.int32)
+    gt_off = np.concatenate([[0], np.cumsum([len(g["gt"]) for g in groups])]).astype(np.int32)
+    n_rows = int(est_off[-1])
+    rows = np.array([e for g in groups for e in g["est"]], np.int64)
+    stages = _Stages(stage_ms is not None)
+    lib = _lib.load()
+    with torch.cuda.device(device):
+        stream = torch.cuda.current_stream(device).cuda_stream
+        mssd = torch.empty(max(n_pairs, 1), device=device)
+        mspd = torch.empty(max(n_pairs, 1), device=device)
+        if n_pairs:
+            meshes = [read_ply(os.path.join(setup["mdir"], f"obj_{o:06d}.ply")) for o in objects]
+            vo = np.concatenate([[0], np.cumsum([len(m["vertices"]) for m in meshes])]).astype(np.int32)
+            vertices = torch.as_tensor(np.concatenate([m["vertices"] for m in meshes]), device=device).contiguous()
+            sym = [symmetry_transforms(info[o]) for o in objects]
+            so = np.concatenate([[0], np.cumsum([len(s) for s in sym])]).astype(np.int32)
+            syms = torch.as_tensor(np.concatenate(sym), dtype=torch.float32, device=device).contiguous()
+            K = torch.as_tensor(np.stack([scenes[s]["K"][im] for s, im in setup["images"]]), dtype=torch.float32,
+                                device=device).contiguous()
+            pose_of_est = {e: _pose(res[e]["R"], res[e]["t"]) for e in set(rows.tolist())}
+            pose_est = np.stack([pose_of_est[e] for e in pairs["est"].tolist()]).astype(np.float32)
+            pose_gt = np.stack([_pose(scenes[groups[gi]["scene_id"]]["gt"][groups[gi]["im_id"]][k]["R"],
+                                      scenes[groups[gi]["scene_id"]]["gt"][groups[gi]["im_id"]][k]["t"])
+                                for gi, k in zip(pairs["group"].tolist(), pairs["gt"].tolist())]).astype(np.float32)
+            pair_obj = np.array([oidx[groups[gi]["obj_id"]] for gi in pairs["group"].tolist()], np.int32)
+            t = lambda a: torch.as_tensor(np.ascontiguousarray(a), device=device)
+            obj_d, frame_d = t(pair_obj), t(pairs["frame"].astype(np.int32))
+            pe_d, pg_d = t(pose_est), t(pose_gt)
+            vo_c, so_c = (C.c_int32 * len(vo))(*vo.tolist()), (C.c_int32 * len(so))(*so.tolist())
+            done = stages.mark("mssd_mspd")
+            for p0 in range(0, n_pairs, MAX_PAIRS_PER_CALL):
+                n = min(MAX_PAIRS_PER_CALL, n_pairs - p0)
+                check(lib.gp_bop_mssd_mspd(n, n_obj, obj_d[p0:].data_ptr(), vo_c, vertices.data_ptr(), so_c,
+                                           syms.data_ptr(), K.shape[0], K.data_ptr(), frame_d[p0:].data_ptr(),
+                                           pe_d[p0:].data_ptr(), pg_d[p0:].data_ptr(), mssd[p0:].data_ptr(),
+                                           mspd[p0:].data_ptr(), stream))
+            if done is not None:
+                done.record()
+        ap = np.zeros((n_obj, 2, T))
+        labels = np.zeros((0, 2, T), np.int8)
+        if n_rows:
+            thr = np.zeros((n_obj, 2, T))
+            for k, o in enumerate(objects):
+                thr[k, 0] = np.asarray(theta_mssd) * info[o]["diameter"]
+                thr[k, 1] = np.asarray(theta_mspd) * r
+            group_obj = np.array([oidx[g["obj_id"]] for g in groups], np.int32)
+            valid = torch.as_tensor(np.concatenate([g["valid"] for g in groups]).astype(np.uint8).reshape(-1),
+                                    device=device)
+            if valid.numel() == 0:
+                valid = torch.zeros(1, dtype=torch.uint8, device=device)
+            ws = torch.empty(8 * thr.size + _lib.BOP_MATCH_GROUP_BYTES * len(groups), dtype=torch.uint8, device=device)
+            lab_d = torch.empty(n_rows, 2, T, dtype=torch.int8, device=device)
+            thr = np.ascontiguousarray(thr)
+            done = stages.mark("match")
+            check(lib.gp_bop_match(len(groups), n_obj, T, _int32p(est_off), _int32p(gt_off), _int32p(group_obj),
+                                   thr.ctypes.data_as(C.POINTER(C.c_double)), mssd.data_ptr(), mspd.data_ptr(),
+                                   valid.data_ptr(), ws.data_ptr(), lab_d.data_ptr(), stream))
+            if done is not None:
+                done.record()
+            # every kept estimate of an object over all images, by descending score, csv order on ties (stable)
+            row_obj = np.array([oidx[g["obj_id"]] for g in groups for _ in g["est"]], np.int64)
+            score = np.array([res[e]["score"] for e in rows.tolist()], np.float64)
+            order = np.lexsort((rows, -score, row_obj)).astype(np.int32)
+            rank_off = np.concatenate([[0], np.cumsum(np.bincount(row_obj, minlength=n_obj))]).astype(np.int32)
+            nv = np.array([setup["n_valid"][o] for o in objects], np.int32)
+            rec = np.ascontiguousarray(RECALL_THRESHOLDS, np.float64)
+            rank_d = torch.as_tensor(order, device=device)
+            ap_d = torch.empty(n_obj, 2, T, dtype=torch.float64, device=device)
+            done = stages.mark("ap")
+            check(lib.gp_bop_average_precision(n_obj, T, n_rows, lab_d.data_ptr(), _int32p(rank_off), rank_d.data_ptr(),
+                                               _int32p(nv), len(rec), rec.ctypes.data_as(C.POINTER(C.c_double)),
+                                               ap_d.data_ptr(), stream))
+            if done is not None:
+                done.record()
+            ap, labels = ap_d.cpu().numpy(), lab_d.cpu().numpy()
+        errors = dict(group=pairs["group"], est=pairs["est"], gt=pairs["gt"], mssd=mssd[:n_pairs].cpu().numpy(),
+                      mspd=mspd[:n_pairs].cpu().numpy())
+    if stage_ms is not None:
+        stage_ms.update(stages.totals())
+    ap_mssd, ap_mspd = np.ascontiguousarray(ap[:, 0]), np.ascontiguousarray(ap[:, 1])
+    map_mssd, map_mspd = float(np.mean(ap_mssd)), float(np.mean(ap_mspd))
+    out = dict(map=(map_mssd + map_mspd) / 2.0, map_mssd=map_mssd, map_mspd=map_mspd, ap_mssd=ap_mssd, ap_mspd=ap_mspd,
+               objects=list(objects), average_time_per_image=average_time_per_image(res), errors=errors,
+               labels=labels, rows=rows)
+    if out_dir is not None:
+        os.makedirs(out_dir, exist_ok=True)
+        scores = {"bop24_mAP": out["map"], "bop24_mAP_mssd": map_mssd, "bop24_mAP_mspd": map_mspd,
+                  "bop24_average_time_per_image": out["average_time_per_image"]}
+        with open(os.path.join(out_dir, "scores_bop24.json"), "w") as f:
+            json.dump(scores, f, indent=2)
+    return out
+
+
 def main(argv=None):
-    ap = argparse.ArgumentParser(description="BOP 2019 pose-error evaluation (VSD, MSSD, MSPD, AR) on the GPU")
+    ap = argparse.ArgumentParser(description="BOP pose-error evaluation on the GPU: the BOP 2019 localization task "
+                                             "(VSD, MSSD, MSPD, AR) or the BOP 2024 6D-detection task (MSSD, MSPD, mAP)")
     ap.add_argument("--results", required=True, help="BOP results csv")
     ap.add_argument("--dataset-dir", required=True)
     ap.add_argument("--split", default="test")
-    ap.add_argument("--out", default=None, help="directory for scores_bop19.json (default: next to the csv)")
+    ap.add_argument("--task", choices=("localization", "detection"), default="localization")
+    ap.add_argument("--out", default=None, help="directory for scores_bop19.json / scores_bop24.json (default: next to "
+                                                "the csv)")
     a = ap.parse_args(argv)
     out_dir = a.out if a.out is not None else os.path.dirname(os.path.abspath(a.results))
+    if a.task == "detection":
+        res = evaluate_detection(a.results, a.dataset_dir, a.split, out_dir=out_dir)
+        print(json.dumps({k: res[k] for k in ("map", "map_mssd", "map_mspd", "objects", "average_time_per_image")}))
+        return
     res = evaluate(a.results, a.dataset_dir, a.split, out_dir=out_dir)
     print(json.dumps({k: res[k] for k in ("ar", "ar_vsd", "ar_mssd", "ar_mspd", "n_targets",
                                           "average_time_per_image")}))

@@ -24,8 +24,37 @@
 //  over vertices is taken on the squared terms, then one sqrt, then the min over transforms with an atomicMin on the
 //  float bits: every value is >= 0 or NaN, so the unsigned bit order is the float order with NaN last, and both the
 //  max and the min are exact and independent of the schedule.
+//
+// Row f8: the BOP 2024 6D-detection score (the toolkit's eval_bop24_pose.py that the reference's README points to for
+// `test_setting: detection` runs), with COCO's rules for ranking, ignored ground truths and interpolated precision
+// (Lin et al., "Microsoft COCO: Common Objects in Context", ECCV 2014).  This is this repository's statement of it; it is
+// unverified against eval_bop24_pose.py.  The host side (gigapose_b200/bop_eval.py, prepare_detection) keeps the
+// max_estimates_per_image highest-scoring estimates of each target image (stable: csv order on ties), calls a ground
+// truth valid when its visib_fract >= 0.1 and ignored otherwise, evaluates the objects with at least one valid ground
+// truth, and computes MSSD / MSPD of every (kept estimate, ground truth of its object in its image) pair with
+// gp_bop_mssd_mspd.  Thresholds are fp64 (theta x diameter, theta x width / 640), computed on the host.
+//  gp_bop_match, one warp per (group = (image, object), metric, threshold): the group's estimates in descending score
+//  order (csv order on ties), each in turn:
+//    1. takes the unmatched valid ground truth with the smallest double(err) < thr (the lowest index on a tie): TP;
+//    2. else takes the unmatched ignored ground truth with the smallest double(err) < thr (lowest index): ignored;
+//    3. else FP.
+//  A NaN error fails `<` and never matches.  Lane l owns the ground truths j = 32 c + l and keeps their taken flags as
+//  bit c of one register (hence at most 32 x 32 ground truths per group); the arg-min is a butterfly on (error, index).
+//  gp_bop_average_precision, one CTA per (object, metric, threshold) over the object's estimates ranked by score over
+//  all images (a host stable argsort): inclusive integer block scans of TP and FP (ignored estimates keep their rank and
+//  add to neither), then per rank, in fp64, recall = TP / n_valid and precision = TP / ((TP + FP) + 2^-52), each one
+//  IEEE operation (__ddiv_rn / __dadd_rn).  The COCO interpolation q_k = max { precision_j : j >= first rank with
+//  recall >= r_k } (0 when no rank reaches r_k) equals max { precision_j : recall_j >= r_k } because the recall is
+//  non-decreasing, so each rank binary-searches c_j = #{k : r_k <= recall_j} and takes an atomicMax of its precision
+//  bits into slot c_j (precisions are >= 0, so the unsigned bit order is the double order and the max is exact); a
+//  suffix max over the slots gives q_k = max over slots c > k.  AP = (((q_0 + q_1) + q_2) + ... + q_{K-1}) / K in fp64,
+//  summed on one thread.  Every step is an integer operation, an exact max or one rounded fp64 operation, so
+//  oracle/bop24_port.py (detection_labels, average_precision) restates it bit for bit.
 #include "../../include/gigapose_b200.h"
 #include "gigapose_kernels.h"
+
+#include <cstring>
+#include <vector>
 
 using gp::fail;
 
@@ -198,6 +227,145 @@ mssd_mspd_kernel(int n_objects, const int32_t* __restrict__ obj_idx, ObjectTable
 
 constexpr int kMaxSide = 8192;
 
+// ---------------------------------------------------------------------------------------------------- row f8
+struct MatchGroup {                   // GP_BOP_MATCH_GROUP_BYTES; gp_bop_match copies one per group into its workspace
+  long long err0;                     // first error of the group's dense [n_est, n_gt] block
+  int32_t est0, n_est, gt0, n_gt, obj, pad;
+};
+static_assert(sizeof(MatchGroup) == GP_BOP_MATCH_GROUP_BYTES, "MatchGroup layout");
+
+// arg-min over the warp of (d, j), the lower j on equal d; every lane ends with the same pair
+__device__ __forceinline__ void warp_argmin(double& d, int& j) {
+#pragma unroll
+  for (int o = 16; o; o >>= 1) {
+    const double d2 = __shfl_xor_sync(0xffffffffu, d, o);
+    const int j2 = __shfl_xor_sync(0xffffffffu, j, o);
+    if (d2 < d || (d2 == d && j2 < j)) { d = d2; j = j2; }
+  }
+}
+
+constexpr int kNone = 0x7fffffff;
+
+__global__ void __launch_bounds__(kThreads)
+match_kernel(long long n_warps, int n_theta, const MatchGroup* __restrict__ groups, const double* __restrict__ thr,
+             const float* __restrict__ mssd, const float* __restrict__ mspd, const uint8_t* __restrict__ gt_valid,
+             int8_t* __restrict__ labels) {
+  const long long w = ((long long)blockIdx.x * kThreads + threadIdx.x) >> 5;
+  const int lane = threadIdx.x & 31;
+  if (w >= n_warps) return;                                  // whole warps: kThreads is a multiple of 32
+  const int g = (int)(w / (2 * n_theta)), m = (int)(w / n_theta) & 1, t = (int)(w % n_theta);
+  const MatchGroup G = groups[g];
+  const double th = thr[((size_t)G.obj * 2 + m) * n_theta + t];
+  const float* err = (m == 0 ? mssd : mspd) + G.err0;
+  const int chunks = (G.n_gt + 31) >> 5;
+  unsigned valid = 0u, taken = 0u;                           // bit c: ground truth 32 c + lane
+  for (int c = 0; c < chunks; ++c) {
+    const int j = 32 * c + lane;
+    if (j < G.n_gt && gt_valid[G.gt0 + j]) valid |= 1u << c;
+  }
+  for (int a = 0; a < G.n_est; ++a) {
+    const float* row = err + (long long)a * G.n_gt;
+    double dv = __longlong_as_double(0x7ff0000000000000ll), di = dv;
+    int jv = kNone, ji = kNone;
+    for (int c = 0; c < chunks; ++c) {                       // ascending j per lane: strict < keeps the lowest
+      const int j = 32 * c + lane;
+      if (j >= G.n_gt || ((taken >> c) & 1u)) continue;
+      const double d = (double)row[j];
+      if (!(d < th)) continue;
+      if ((valid >> c) & 1u) {
+        if (d < dv) { dv = d; jv = j; }
+      } else if (d < di) {
+        di = d;
+        ji = j;
+      }
+    }
+    warp_argmin(dv, jv);
+    int label = GP_BOP_LABEL_FP, take = kNone;
+    if (jv != kNone) {
+      label = GP_BOP_LABEL_TP;
+      take = jv;
+    } else {
+      warp_argmin(di, ji);                                   // warp-uniform branch: jv is the same on every lane
+      if (ji != kNone) { label = GP_BOP_LABEL_IGNORED; take = ji; }
+    }
+    if (take != kNone && (take & 31) == lane) taken |= 1u << (take >> 5);
+    if (lane == 0) labels[((size_t)(G.est0 + a) * 2 + m) * n_theta + t] = (int8_t)label;
+  }
+}
+
+struct ApTables {                     // host tables, by value: object o ranks rank[off[o] .. off[o + 1])
+  int32_t rank_off[GP_BOP_MAX_OBJECTS + 1];
+  int32_t n_valid[GP_BOP_MAX_OBJECTS];
+  double recall[GP_BOP_MAX_RECALL];
+};
+
+__global__ void __launch_bounds__(kThreads)
+ap_kernel(int n_theta, int n_est, const int8_t* __restrict__ labels, const int32_t* __restrict__ rank, int n_recall,
+          ApTables tab, double* __restrict__ ap) {
+  __shared__ unsigned long long best[GP_BOP_MAX_RECALL + 1];  // slot c: max precision bits of ranks with c_j = c
+  __shared__ double rthr[GP_BOP_MAX_RECALL];
+  __shared__ int wsum[2][kWarps];
+  __shared__ int bad;
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int o = blockIdx.x / (2 * n_theta), m = (blockIdx.x / n_theta) & 1, t = blockIdx.x % n_theta;
+  for (int c = tid; c <= n_recall; c += kThreads) best[c] = 0ull;
+  for (int c = tid; c < n_recall; c += kThreads) rthr[c] = tab.recall[c];
+  if (tid == 0) bad = 0;
+  __syncthreads();
+  const int r0 = tab.rank_off[o], n = tab.rank_off[o + 1] - r0;
+  const double nv = (double)tab.n_valid[o];
+  int carry_tp = 0, carry_fp = 0;
+  for (int base = 0; base < n; base += kThreads) {
+    const int i = base + tid;
+    int tp = 0, fp = 0;
+    if (i < n) {
+      const int e = rank[r0 + i];
+      if (e < 0 || e >= n_est) {
+        bad = 1;
+      } else {
+        const int L = labels[((size_t)e * 2 + m) * n_theta + t];
+        tp = L == GP_BOP_LABEL_TP;
+        fp = L == GP_BOP_LABEL_FP;
+      }
+    }
+#pragma unroll
+    for (int d = 1; d < 32; d <<= 1) {                       // inclusive warp scans
+      const int a = __shfl_up_sync(0xffffffffu, tp, d), b = __shfl_up_sync(0xffffffffu, fp, d);
+      if (lane >= d) { tp += a; fp += b; }
+    }
+    if (lane == 31) { wsum[0][warp] = tp; wsum[1][warp] = fp; }
+    __syncthreads();
+    int tile_tp = 0, tile_fp = 0;
+#pragma unroll
+    for (int w = 0; w < kWarps; ++w) {
+      if (w < warp) { tp += wsum[0][w]; fp += wsum[1][w]; }
+      tile_tp += wsum[0][w];
+      tile_fp += wsum[1][w];
+    }
+    __syncthreads();                                         // wsum is rewritten by the next tile
+    if (i < n) {
+      const int TP = carry_tp + tp, FP = carry_fp + fp;
+      const double rc = __ddiv_rn((double)TP, nv);
+      const double pr = __ddiv_rn((double)TP, __dadd_rn((double)(TP + FP), 0x1p-52));
+      int lo = 0, hi = n_recall;                             // c_j = #{k : r_k <= recall_j}
+      while (lo < hi) {
+        const int mid = (lo + hi) >> 1;
+        if (rthr[mid] <= rc) lo = mid + 1; else hi = mid;
+      }
+      if (lo > 0) atomicMax(&best[lo], (unsigned long long)__double_as_longlong(pr));
+    }
+    carry_tp += tile_tp;
+    carry_fp += tile_fp;
+  }
+  __syncthreads();
+  if (tid == 0) {
+    for (int c = n_recall - 1; c >= 1; --c) best[c] = max(best[c], best[c + 1]);
+    double sum = 0.0;
+    for (int k = 0; k < n_recall; ++k) sum = __dadd_rn(sum, __longlong_as_double((long long)best[k + 1]));
+    ap[blockIdx.x] = bad ? __longlong_as_double(0x7ff8000000000000ll) : __ddiv_rn(sum, (double)n_recall);
+  }
+}
+
 }  // namespace
 
 extern "C" int gp_bop_vsd(int n_pairs, int n_frames, int height, int width, const float* depth_test, const float* K,
@@ -258,5 +426,85 @@ extern "C" int gp_bop_mssd_mspd(int n_pairs, int n_objects, const int32_t* obj_i
   GP_CUDA(gp::launch_ex(mssd_mspd_kernel, dim3(n_pairs, (max_syms + kSymPerCta - 1) / kSymPerCta), kThreads, 0, st, 1,
                         false, n_objects, obj_idx, tab, vertices, syms, n_frames, K, frame_idx, pose_est, pose_gt, mssd,
                         mspd));
+  return GP_OK;
+}
+
+static bool check_offsets(const int32_t* off, int n) {
+  if (off[0] != 0) return false;
+  for (int i = 1; i <= n; ++i)
+    if (off[i] < off[i - 1]) return false;
+  return true;
+}
+
+extern "C" int gp_bop_match(int n_groups, int n_objects, int n_theta, const int32_t* est_offsets,
+                            const int32_t* gt_offsets, const int32_t* group_obj, const double* thresholds,
+                            const float* mssd, const float* mspd, const uint8_t* gt_valid, void* workspace,
+                            int8_t* labels, void* stream) {
+  if (n_groups < 1) return fail(GP_ERR_INVALID, "n_groups %d must be >= 1", n_groups);
+  if (n_objects < 1 || n_objects > GP_BOP_MAX_OBJECTS)
+    return fail(GP_ERR_INVALID, "n_objects %d outside [1, %d]", n_objects, GP_BOP_MAX_OBJECTS);
+  if (n_theta < 1 || n_theta > GP_BOP_MAX_TAU)
+    return fail(GP_ERR_INVALID, "n_theta %d outside [1, %d]", n_theta, GP_BOP_MAX_TAU);
+  if (!est_offsets || !gt_offsets || !group_obj || !thresholds) return fail(GP_ERR_INVALID, "null host table");
+  if (!check_offsets(est_offsets, n_groups) || !check_offsets(gt_offsets, n_groups))
+    return fail(GP_ERR_INVALID, "bad offsets: they must start at 0 and not decrease");
+  const size_t n_thr = (size_t)n_objects * 2 * n_theta;
+  for (size_t i = 0; i < n_thr; ++i)
+    if (!isfinite(thresholds[i])) return fail(GP_ERR_INVALID, "thresholds[%zu] is not finite", i);
+  if (!mssd || !mspd || !gt_valid || !workspace || !labels) return fail(GP_ERR_INVALID, "null argument");
+  if (reinterpret_cast<uintptr_t>(workspace) % 8) return fail(GP_ERR_INVALID, "workspace must be 8-byte aligned");
+  std::vector<unsigned char> host(n_thr * sizeof(double) + (size_t)n_groups * sizeof(MatchGroup));
+  memcpy(host.data(), thresholds, n_thr * sizeof(double));
+  MatchGroup* tab = reinterpret_cast<MatchGroup*>(host.data() + n_thr * sizeof(double));
+  long long err0 = 0;
+  for (int g = 0; g < n_groups; ++g) {
+    const int n_gt = gt_offsets[g + 1] - gt_offsets[g];
+    if (n_gt > GP_BOP_MAX_GT_PER_GROUP)
+      return fail(GP_ERR_INVALID, "group %d has %d ground truths, more than %d", g, n_gt, GP_BOP_MAX_GT_PER_GROUP);
+    if (group_obj[g] < 0 || group_obj[g] >= n_objects)
+      return fail(GP_ERR_INVALID, "group_obj[%d] = %d outside [0, %d)", g, group_obj[g], n_objects);
+    tab[g] = MatchGroup{err0, est_offsets[g], est_offsets[g + 1] - est_offsets[g], gt_offsets[g], n_gt, group_obj[g], 0};
+    err0 += (long long)tab[g].n_est * n_gt;
+  }
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  GP_CUDA(cudaMemcpyAsync(workspace, host.data(), host.size(), cudaMemcpyHostToDevice, st));
+  const double* thr_dev = static_cast<const double*>(workspace);
+  const MatchGroup* tab_dev = reinterpret_cast<const MatchGroup*>(static_cast<const unsigned char*>(workspace) +
+                                                                  n_thr * sizeof(double));
+  const long long n_warps = (long long)n_groups * 2 * n_theta;
+  GP_CUDA(gp::launch_ex(match_kernel, (unsigned)((n_warps + kWarps - 1) / kWarps), kThreads, 0, st, 1, false, n_warps,
+                        n_theta, tab_dev, thr_dev, mssd, mspd, gt_valid, labels));
+  return GP_OK;
+}
+
+extern "C" int gp_bop_average_precision(int n_objects, int n_theta, int n_est, const int8_t* labels,
+                                        const int32_t* rank_offsets, const int32_t* rank, const int32_t* n_valid,
+                                        int n_recall, const double* recall_thresholds, double* ap, void* stream) {
+  if (n_objects < 1 || n_objects > GP_BOP_MAX_OBJECTS)
+    return fail(GP_ERR_INVALID, "n_objects %d outside [1, %d]", n_objects, GP_BOP_MAX_OBJECTS);
+  if (n_theta < 1 || n_theta > GP_BOP_MAX_TAU)
+    return fail(GP_ERR_INVALID, "n_theta %d outside [1, %d]", n_theta, GP_BOP_MAX_TAU);
+  if (n_est < 1) return fail(GP_ERR_INVALID, "n_est %d must be >= 1", n_est);
+  if (n_recall < 1 || n_recall > GP_BOP_MAX_RECALL)
+    return fail(GP_ERR_INVALID, "n_recall %d outside [1, %d]", n_recall, GP_BOP_MAX_RECALL);
+  if (!rank_offsets || !n_valid || !recall_thresholds) return fail(GP_ERR_INVALID, "null host table");
+  if (!check_offsets(rank_offsets, n_objects))
+    return fail(GP_ERR_INVALID, "bad rank offsets: they must start at 0 and not decrease");
+  ApTables tab;
+  for (int o = 0; o <= GP_BOP_MAX_OBJECTS; ++o) tab.rank_off[o] = rank_offsets[min(o, n_objects)];
+  for (int o = 0; o < GP_BOP_MAX_OBJECTS; ++o) {
+    tab.n_valid[o] = o < n_objects ? n_valid[o] : 1;
+    if (tab.n_valid[o] < 1) return fail(GP_ERR_INVALID, "n_valid[%d] = %d must be >= 1", o, tab.n_valid[o]);
+  }
+  for (int k = 0; k < GP_BOP_MAX_RECALL; ++k) {
+    tab.recall[k] = k < n_recall ? recall_thresholds[k] : 0.0;
+    if (k < n_recall && !isfinite(tab.recall[k]))
+      return fail(GP_ERR_INVALID, "recall_thresholds[%d] is not finite", k);
+    if (k > 0 && k < n_recall && tab.recall[k] < tab.recall[k - 1])
+      return fail(GP_ERR_INVALID, "recall_thresholds must not decrease (at %d)", k);
+  }
+  if (!labels || !rank || !ap) return fail(GP_ERR_INVALID, "null argument");
+  GP_CUDA(gp::launch_ex(ap_kernel, n_objects * 2 * n_theta, kThreads, 0, static_cast<cudaStream_t>(stream), 1, false,
+                        n_theta, n_est, labels, rank, n_recall, tab, ap));
   return GP_OK;
 }

@@ -328,6 +328,40 @@ int gp_bop_mssd_mspd(int n_pairs, int n_objects, const int32_t* obj_idx, const i
                      const int32_t* frame_idx, const float* pose_est, const float* pose_gt, float* mssd, float* mspd,
                      void* stream);
 
+/* --- row f8: BOP 2024 6D-detection score (the toolkit's eval_bop24_pose.py, which the reference's README names for
+ * `test_setting: detection` runs): greedy matching with ignored ground truths and COCO average precision over MSSD /
+ * MSPD.  The full contract, with the fp64 operation order, is the header comment of gigapose_b200/csrc/bop_eval.cu.
+ * Needs no handle; the two calls run in stream order with no host synchronisation between them. ------------------- */
+#define GP_BOP_MAX_GT_PER_GROUP 1024   /* ground truths per (image, object) group in gp_bop_match (32 x 32 flags) */
+#define GP_BOP_MAX_RECALL 128          /* recall thresholds per gp_bop_average_precision call */
+#define GP_BOP_MATCH_GROUP_BYTES 32    /* workspace bytes per group of gp_bop_match */
+#define GP_BOP_LABEL_FP 0
+#define GP_BOP_LABEL_TP 1
+#define GP_BOP_LABEL_IGNORED 2
+/* Greedy matching of n_groups (image, object) groups for the 2 metrics (0 = MSSD, 1 = MSPD) x n_theta thresholds.
+ *   HOST tables: est_offsets / gt_offsets i32 [n_groups + 1] (0 first, non-decreasing): group g owns the estimate rows
+ *   [est_offsets[g], est_offsets[g + 1]), in descending score order, and the ground truths [gt_offsets[g],
+ *   gt_offsets[g + 1]) (at most GP_BOP_MAX_GT_PER_GROUP); group_obj i32 [n_groups] in [0, n_objects);
+ *   thresholds f64 [n_objects, 2, n_theta], finite (1 <= n_theta <= GP_BOP_MAX_TAU).
+ *   Device: mssd / mspd f32 [sum_g n_est_g * n_gt_g], each group a dense row-major [n_est, n_gt] block, the groups in
+ *   order; gt_valid u8 [gt_offsets[n_groups]] (1 = valid, 0 = ignored); workspace of 8 * 2 * n_objects * n_theta +
+ *   GP_BOP_MATCH_GROUP_BYTES * n_groups bytes, 8-byte aligned (the host tables are copied there in stream order
+ *   before the call returns).
+ * Output labels i8 [est_offsets[n_groups], 2, n_theta]: GP_BOP_LABEL_FP / _TP / _IGNORED. */
+int gp_bop_match(int n_groups, int n_objects, int n_theta, const int32_t* est_offsets, const int32_t* gt_offsets,
+                 const int32_t* group_obj, const double* thresholds, const float* mssd, const float* mspd,
+                 const uint8_t* gt_valid, void* workspace, int8_t* labels, void* stream);
+/* COCO average precision per (object, metric, threshold) from the labels of gp_bop_match.
+ *   labels i8 [n_est, 2, n_theta] (device); rank i32 (device): object o's estimate rows ranked by descending score
+ *   over all images at rank[rank_offsets[o] .. rank_offsets[o + 1]) (HOST offsets i32 [n_objects + 1], 0 first,
+ *   non-decreasing); n_valid i32 [n_objects] (HOST, each >= 1) valid ground truths per object; recall_thresholds
+ *   (HOST f64 [n_recall], finite, non-decreasing, 1 <= n_recall <= GP_BOP_MAX_RECALL).
+ * Output ap f64 [n_objects, 2, n_theta] (0 for an object without estimates; NaN if a rank index is outside
+ * [0, n_est)). */
+int gp_bop_average_precision(int n_objects, int n_theta, int n_est, const int8_t* labels, const int32_t* rank_offsets,
+                             const int32_t* rank, const int32_t* n_valid, int n_recall, const double* recall_thresholds,
+                             double* ap, void* stream);
+
 /* --- row f6: depth refinement of the coarse poses (MegaPose's ICPRefiner, src/megapose/inference/icp_refiner.py:134-287,
  * with a GPU point-to-plane ICP in place of OpenCV's ppf_match_3d_ICP).  The full contract is the header comment of
  * gigapose_b200/csrc/depth_icp.cu.  Needs no handle. ------------------------------------------------------------- */
