@@ -16,6 +16,7 @@ Usage:
 from __future__ import annotations
 
 import argparse
+import contextlib
 import ctypes as C
 import json
 import os
@@ -40,6 +41,7 @@ MAX_SYM_DISC_STEP = 0.01        # continuous symmetries: the farthest vertex mov
 VISIB_GT_MIN = 0.1              # ground truths less visible than this are neither targets nor matchable
 Z_NEAR = 10.0                   # renders: near plane, model unit
 WORKSPACE_BYTES = 1 << 30       # device memory per chunk of images: measured depth, renders and the render keys
+MAX_PAIRS_PER_CALL = 1 << 18    # pairs per gp_bop_mssd_mspd call: ~140 B of poses, indices and errors each, ~37 MB
 
 
 class BopEvalError(ValueError):
@@ -180,6 +182,17 @@ def recalls(groups, n_targets, taus=TAUS, theta_vsd=THETA_VSD, theta_mssd=THETA_
 
 
 # ---------------------------------------------------------------------------------------------------- set-up
+def _scene(scenes, dataset_dir, split, scene_id, im_id):
+    """scenes[scene_id] (a `load_scene` dict), loaded on first use; refuses a target image that the scene's
+    scene_gt.json or scene_camera.json lacks."""
+    if scene_id not in scenes:
+        scenes[scene_id] = load_scene(dataset_dir, split, scene_id)
+    sc = scenes[scene_id]
+    if im_id not in sc["gt"] or im_id not in sc["K"]:
+        raise BopEvalError(f"target image {scene_id}/{im_id} is not in scene_gt.json / scene_camera.json")
+    return sc
+
+
 def prepare(results, dataset_dir, split="test", targets_name="test_targets_bop19.json"):
     """Host side: reads the dataset, keeps the top inst_count estimates per target by score and lists every
     (estimate, ground truth) pair of the same object in an image.  -> dict with `images` [(scene, im)], `targets`,
@@ -188,6 +201,8 @@ def prepare(results, dataset_dir, split="test", targets_name="test_targets_bop19
     targets = load_targets(dataset_dir, targets_name)
     mdir = models_dir(dataset_dir)
     info = load_models_info(mdir)
+    if not targets:
+        raise BopEvalError(f"{os.path.join(dataset_dir, targets_name)} lists no targets")
     by_key = {}
     for i, res in enumerate(results):
         by_key.setdefault((res["scene_id"], res["im_id"], res["obj_id"]), []).append(i)
@@ -197,11 +212,7 @@ def prepare(results, dataset_dir, split="test", targets_name="test_targets_bop19
         s, im, o = t["scene_id"], t["im_id"], t["obj_id"]
         if o not in info:
             raise BopEvalError(f"object {o} of a target is not in {mdir}/models_info.json")
-        if s not in scenes:
-            scenes[s] = load_scene(dataset_dir, split, s)
-        sc = scenes[s]
-        if im not in sc["gt"] or im not in sc["K"]:
-            raise BopEvalError(f"target image {s}/{im} is not in scene_gt.json / scene_camera.json")
+        sc = _scene(scenes, dataset_dir, split, s, im)
         if (s, im) not in images:
             images.append((s, im))
         ests = by_key.get((s, im, o), [])
@@ -222,18 +233,22 @@ def _pose(R, t):
 
 
 class _Stages:
-    """CUDA events around each stage of each chunk; milliseconds summed per stage after a synchronise."""
+    """CUDA events around each stage of each chunk (`with stages(name): ...`); milliseconds summed per stage after a
+    synchronise.  Disabled, it records nothing."""
 
     def __init__(self, enabled):
         self.enabled, self.marks = enabled, []
 
-    def mark(self, name):
+    @contextlib.contextmanager
+    def __call__(self, name):
         if not self.enabled:
-            return None
+            yield
+            return
         ev = (torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True))
         ev[0].record()
         self.marks.append((name, ev))
-        return ev[1]
+        yield
+        ev[1].record()
 
     def totals(self):
         torch.cuda.synchronize()
@@ -266,17 +281,51 @@ def vsd(depth_test, K, frame_idx, est_depth, est_boxes, est_idx, gt_depth, gt_bo
 
 
 def mssd_mspd(obj_idx, vertex_offsets, vertices, sym_offsets, syms, K, frame_idx, pose_est, pose_gt):
-    """gp_bop_mssd_mspd on device tensors (offsets are host int sequences) -> mssd, mspd f32 [n]."""
+    """gp_bop_mssd_mspd on device tensors (offsets are host int sequences), at most MAX_PAIRS_PER_CALL pairs per call
+    and no call for no pairs -> mssd, mspd f32 [n]."""
     n = obj_idx.shape[0]
     mssd = torch.empty(n, device=vertices.device)
     mspd = torch.empty(n, device=vertices.device)
     vo = (C.c_int32 * len(vertex_offsets))(*vertex_offsets)
     so = (C.c_int32 * len(sym_offsets))(*sym_offsets)
-    check(_lib.load().gp_bop_mssd_mspd(n, len(vertex_offsets) - 1, obj_idx.data_ptr(), vo, vertices.data_ptr(), so,
-                                       syms.data_ptr(), K.shape[0], K.data_ptr(), frame_idx.data_ptr(),
-                                       pose_est.data_ptr(), pose_gt.data_ptr(), mssd.data_ptr(), mspd.data_ptr(),
-                                       torch.cuda.current_stream(vertices.device).cuda_stream))
+    lib, stream = _lib.load(), torch.cuda.current_stream(vertices.device).cuda_stream
+    # per-pair arrays as (address, bytes per pair): six slices per call would cost more host time than the launch
+    rows = [(t.data_ptr(), t.stride(0) * t.element_size()) for t in (obj_idx, frame_idx, pose_est, pose_gt, mssd, mspd)]
+    for p0 in range(0, n, MAX_PAIRS_PER_CALL):
+        o, f, pe, pg, a, b = (ptr + p0 * step for ptr, step in rows)
+        check(lib.gp_bop_mssd_mspd(min(MAX_PAIRS_PER_CALL, n - p0), len(vertex_offsets) - 1, o, vo, vertices.data_ptr(),
+                                   so, syms.data_ptr(), K.shape[0], K.data_ptr(), f, pe, pg, a, b, stream))
     return mssd, mspd
+
+
+def _object_tables(setup, obj_ids, device):
+    """Reads each object's PLY once.  -> (host meshes (`read_ply` dicts), the objects' vertices f32 [sum V, 3] and
+    symmetry transforms f32 [sum S, 4, 4] concatenated on `device`, vertex offsets and symmetry offsets [n_obj + 1]
+    as host ints), in the order of obj_ids: the object tables of gp_bop_mssd_mspd."""
+    meshes = [read_ply(os.path.join(setup["mdir"], f"obj_{o:06d}.ply")) for o in obj_ids]
+    sym = [symmetry_transforms(setup["info"][o]) for o in obj_ids]
+    vertices = torch.as_tensor(np.concatenate([m["vertices"] for m in meshes]), device=device).contiguous()
+    syms = torch.as_tensor(np.concatenate(sym), dtype=torch.float32, device=device).contiguous()
+    vertex_offsets = np.cumsum([0] + [len(m["vertices"]) for m in meshes]).tolist()
+    sym_offsets = np.cumsum([0] + [len(s) for s in sym]).tolist()
+    return meshes, vertices, syms, vertex_offsets, sym_offsets
+
+
+def _pair_rows(groups, group_ids, images):
+    """Every (kept estimate, ground truth) pair of groups[gi] for gi in group_ids, group after group, each group a
+    row-major [n_est, n_gt] block (the layout gp_bop_match reads).  -> dict of int64 arrays over the pairs: group, est
+    (result index), gt (instance index), frame (index of the group's image in `images`)."""
+    frame = {key: f for f, key in enumerate(images)}
+    cols = dict(group=[], est=[], gt=[], frame=[])
+    for gi in group_ids:
+        g = groups[gi]
+        ne, ng = len(g["est"]), len(g["gt"])
+        if ne and ng:
+            cols["group"].append(np.full(ne * ng, gi))
+            cols["est"].append(np.repeat(np.asarray(g["est"], np.int64), ng))
+            cols["gt"].append(np.tile(np.asarray(g["gt"], np.int64), ne))
+            cols["frame"].append(np.full(ne * ng, frame[(g["scene_id"], g["im_id"])]))
+    return {k: np.concatenate(v).astype(np.int64) if v else np.zeros(0, np.int64) for k, v in cols.items()}
 
 
 def compute_errors(setup, device="cuda", delta=None, taus=TAUS, z_near=Z_NEAR, stage_ms=None):
@@ -297,17 +346,10 @@ def compute_errors(setup, device="cuda", delta=None, taus=TAUS, z_near=Z_NEAR, s
         raise BopEvalError(f"at most {_lib.BOP_MAX_OBJECTS} objects per evaluation")
     oidx = {o: i for i, o in enumerate(obj_ids)}
     out = dict(group=[], est=[], gt=[], vsd=[], vsd_counts=[], mssd=[], mspd=[])
-    if not obj_ids:
-        return {k: np.zeros((0,)) for k in out}
     stages = _Stages(stage_ms is not None)
-    meshes = [read_ply(os.path.join(setup["mdir"], f"obj_{o:06d}.ply")) for o in obj_ids]
     with torch.cuda.device(device):
+        meshes, vertices, syms, vo, so = _object_tables(setup, obj_ids, device)
         dms = device_meshes(meshes, device)
-        vo = np.concatenate([[0], np.cumsum([len(m["vertices"]) for m in meshes])]).astype(np.int32)
-        vertices = torch.as_tensor(np.concatenate([m["vertices"] for m in meshes]), device=device).contiguous()
-        sym = [symmetry_transforms(info[o]) for o in obj_ids]
-        so = np.concatenate([[0], np.cumsum([len(s) for s in sym])]).astype(np.int32)
-        syms = torch.as_tensor(np.concatenate(sym), dtype=torch.float32, device=device).contiguous()
         diam = {o: info[o]["diameter"] for o in obj_ids}
         by_image = {}
         for gi, g in enumerate(groups):
@@ -329,9 +371,9 @@ def compute_errors(setup, device="cuda", delta=None, taus=TAUS, z_near=Z_NEAR, s
         key_views = max(1, WORKSPACE_BYTES // 2 // (8 * H * W))
         keys_ws = torch.empty(key_views * 8 * H * W, dtype=torch.uint8, device=device)
         for chunk in chunks:
-            depth_np, K_np = [], []
+            depth_np, K_np, group_ids = [], [], []
             renders = []               # (object, pose [4,4], frame) of every estimate, then every ground truth
-            pair_rows = []             # (group, est id, gt id, frame, est render, gt render)
+            er, gr = {}, {}            # render of each (group, est id) / (group, gt id)
             for f, (s, im) in enumerate(chunk):
                 sc = scenes[s]
                 d = load_depth(setup["dataset_dir"], setup["split"], s, im, sc["depth_scale"][im])
@@ -341,57 +383,47 @@ def compute_errors(setup, device="cuda", delta=None, taus=TAUS, z_near=Z_NEAR, s
                 K_np.append(sc["K"][im])
                 for gi in by_image[(s, im)]:
                     g = groups[gi]
-                    er = []
                     for e in g["est"]:
-                        er.append(len(renders))
+                        er[gi, e] = len(renders)
                         renders.append((g["obj_id"], _pose(results[e]["R"], results[e]["t"]), f))
-                    gr = []
                     for k in g["gt"]:
-                        gr.append(len(renders))
+                        gr[gi, k] = len(renders)
                         renders.append((g["obj_id"], _pose(sc["gt"][im][k]["R"], sc["gt"][im][k]["t"]), f))
-                    for a, e in enumerate(g["est"]):
-                        for b, k in enumerate(g["gt"]):
-                            pair_rows.append((gi, e, k, f, er[a], gr[b]))
-            if not pair_rows:
+                    group_ids.append(gi)
+            rows = _pair_rows(groups, group_ids, chunk)
+            if not len(rows["group"]):
                 continue
-            done = stages.mark("renders")
-            depth_test = torch.as_tensor(np.stack(depth_np), device=device)
-            K = torch.as_tensor(np.stack(K_np), dtype=torch.float32, device=device).contiguous()
-            n_r = len(renders)
-            rdepth = torch.empty(n_r, H, W, device=device)
-            rboxes = torch.empty(n_r, 4, dtype=torch.int64, device=device)
-            poses = torch.as_tensor(np.stack([r[1] for r in renders]), dtype=torch.float32, device=device)
-            batches = {}
-            for i, (o, _, f) in enumerate(renders):          # one call per (object, K) shares the mesh and K
-                batches.setdefault((o, K_np[f].astype(np.float32).tobytes()), []).append(i)
-            for (o, _), idx in batches.items():
-                Kf = K[renders[idx[0]][2]].contiguous()
-                for s0 in range(0, len(idx), key_views):
-                    sel = torch.as_tensor(idx[s0:s0 + key_views], device=device)
-                    d = torch.empty(len(sel), H, W, device=device)
-                    b = torch.empty(len(sel), 4, dtype=torch.int64, device=device)
-                    render_depth(dms[oidx[o]], poses[sel].contiguous(), Kf, H, W, z_near, keys_ws, d, b)
-                    rdepth[sel], rboxes[sel] = d, b
-            if done is not None:
-                done.record()
-            rows = np.array(pair_rows, np.int64)
-            col = lambda j: torch.as_tensor(rows[:, j].astype(np.int32), device=device)
-            fi, ei, gi_ = col(3), col(4), col(5)
-            pair_obj = np.array([oidx[groups[r[0]]["obj_id"]] for r in pair_rows], np.int32)
-            pair_diam = torch.as_tensor(np.array([diam[groups[r[0]]["obj_id"]] for r in pair_rows], np.float32),
-                                        device=device)
-            done = stages.mark("vsd")
-            counts, errs = vsd(depth_test, K, fi, rdepth, rboxes, ei, rdepth, rboxes, gi_, pair_diam, delta, taus)
-            if done is not None:
-                done.record()
-            done = stages.mark("mssd_mspd")
-            mssd, mspd = mssd_mspd(torch.as_tensor(pair_obj, device=device), vo.tolist(), vertices, so.tolist(), syms, K,
-                                   fi, poses[ei.long()].contiguous(), poses[gi_.long()].contiguous())
-            if done is not None:
-                done.record()
-            out["group"].append(rows[:, 0])
-            out["est"].append(rows[:, 1])
-            out["gt"].append(rows[:, 2])
+            with stages("renders"):
+                depth_test = torch.as_tensor(np.stack(depth_np), device=device)
+                K = torch.as_tensor(np.stack(K_np), dtype=torch.float32, device=device).contiguous()
+                n_r = len(renders)
+                rdepth = torch.empty(n_r, H, W, device=device)
+                rboxes = torch.empty(n_r, 4, dtype=torch.int64, device=device)
+                poses = torch.as_tensor(np.stack([r[1] for r in renders]), dtype=torch.float32, device=device)
+                batches = {}
+                for i, (o, _, f) in enumerate(renders):          # one call per (object, K) shares the mesh and K
+                    batches.setdefault((o, K_np[f].astype(np.float32).tobytes()), []).append(i)
+                for (o, _), idx in batches.items():
+                    Kf = K[renders[idx[0]][2]].contiguous()
+                    for s0 in range(0, len(idx), key_views):
+                        sel = torch.as_tensor(idx[s0:s0 + key_views], device=device)
+                        d = torch.empty(len(sel), H, W, device=device)
+                        b = torch.empty(len(sel), 4, dtype=torch.int64, device=device)
+                        render_depth(dms[oidx[o]], poses[sel].contiguous(), Kf, H, W, z_near, keys_ws, d, b)
+                        rdepth[sel], rboxes[sel] = d, b
+            group, est, gt = rows["group"].tolist(), rows["est"].tolist(), rows["gt"].tolist()
+            col = lambda a: torch.as_tensor(np.asarray(a, np.int32), device=device)
+            fi, ei, gi_ = col(rows["frame"]), col([er[p] for p in zip(group, est)]), col([gr[p] for p in zip(group, gt)])
+            pair_obj = np.array([oidx[groups[gi]["obj_id"]] for gi in group], np.int32)
+            pair_diam = torch.as_tensor(np.array([diam[groups[gi]["obj_id"]] for gi in group], np.float32), device=device)
+            with stages("vsd"):
+                counts, errs = vsd(depth_test, K, fi, rdepth, rboxes, ei, rdepth, rboxes, gi_, pair_diam, delta, taus)
+            with stages("mssd_mspd"):
+                mssd, mspd = mssd_mspd(torch.as_tensor(pair_obj, device=device), vo, vertices, so, syms, K, fi,
+                                       poses[ei.long()].contiguous(), poses[gi_.long()].contiguous())
+            out["group"].append(rows["group"])
+            out["est"].append(rows["est"])
+            out["gt"].append(rows["gt"])
             out["vsd"].append(errs.cpu().numpy())
             out["vsd_counts"].append(counts.cpu().numpy())
             out["mssd"].append(mssd.cpu().numpy())
@@ -436,6 +468,15 @@ def average_time_per_image(results):
     return float(np.mean([np.mean(t) for t in per.values()]))
 
 
+def _write_scores(out_dir, name, scores):
+    """out_dir/name as indented JSON; nothing when out_dir is None."""
+    if out_dir is None:
+        return
+    os.makedirs(out_dir, exist_ok=True)
+    with open(os.path.join(out_dir, name), "w") as f:
+        json.dump(scores, f, indent=2)
+
+
 @torch.no_grad()
 def evaluate(results, dataset_dir, split="test", out_dir=None, device="cuda", delta=None, taus=TAUS,
              theta_vsd=THETA_VSD, theta_mssd=THETA_MSSD, theta_mspd=THETA_MSPD,
@@ -446,24 +487,16 @@ def evaluate(results, dataset_dir, split="test", out_dir=None, device="cuda", de
     out_dir/scores_bop19.json with the keys the reference's eval_bop.py reads."""
     setup = prepare(results, dataset_dir, split, targets_name)
     errors = compute_errors(setup, device, delta, taus, stage_ms=stage_ms)
-    H_W = None
-    if setup["images"]:
-        s, im = setup["images"][0]
-        H_W = load_depth(dataset_dir, split, s, im, setup["scenes"][s]["depth_scale"][im]).shape
-    r = (H_W[1] if H_W else 640) / 640.0
+    r = image_width(dataset_dir, split, *setup["images"][0]) / 640.0
     n_targets = int(sum(g["valid"].sum() for g in setup["groups"]))
     rec = recalls(error_groups(setup, errors), n_targets, taus, theta_vsd, theta_mssd, theta_mspd, r)
     ar_vsd, ar_mssd, ar_mspd = float(rec["vsd"].mean()), float(rec["mssd"].mean()), float(rec["mspd"].mean())
     out = dict(ar=(ar_vsd + ar_mssd + ar_mspd) / 3.0, ar_vsd=ar_vsd, ar_mssd=ar_mssd, ar_mspd=ar_mspd,
                recall_vsd=rec["vsd"], recall_mssd=rec["mssd"], recall_mspd=rec["mspd"], n_targets=n_targets,
                average_time_per_image=average_time_per_image(setup["results"]), errors=errors)
-    if out_dir is not None:
-        os.makedirs(out_dir, exist_ok=True)
-        scores = {"bop19_average_recall": out["ar"], "bop19_average_recall_vsd": ar_vsd,
-                  "bop19_average_recall_mssd": ar_mssd, "bop19_average_recall_mspd": ar_mspd,
-                  "bop19_average_time_per_image": out["average_time_per_image"]}
-        with open(os.path.join(out_dir, "scores_bop19.json"), "w") as f:
-            json.dump(scores, f, indent=2)
+    _write_scores(out_dir, "scores_bop19.json", {
+        "bop19_average_recall": out["ar"], "bop19_average_recall_vsd": ar_vsd, "bop19_average_recall_mssd": ar_mssd,
+        "bop19_average_recall_mspd": ar_mspd, "bop19_average_time_per_image": out["average_time_per_image"]})
     return out
 
 
@@ -475,7 +508,6 @@ def evaluate(results, dataset_dir, split="test", out_dir=None, device="cuda", de
 TARGETS_BOP24 = "test_targets_bop24.json"
 MAX_ESTIMATES_PER_IMAGE = 100   # highest scores kept per image (stable: csv order on ties)
 RECALL_THRESHOLDS = np.linspace(0.0, 1.0, 101)                   # COCO's 101 recall points
-MAX_PAIRS_PER_CALL = 1 << 18    # pairs per gp_bop_mssd_mspd call: ~140 B of poses, indices and errors each, ~37 MB
 
 
 def load_target_images(dataset_dir, name=TARGETS_BOP24):
@@ -515,11 +547,8 @@ def prepare_detection(results, dataset_dir, split="test", targets_name=TARGETS_B
     scenes = {}
     n_valid = {}
     for s, im in images:
-        if s not in scenes:
-            scenes[s] = load_scene(dataset_dir, split, s)
-        if im not in scenes[s]["gt"] or im not in scenes[s]["K"]:
-            raise BopEvalError(f"target image {s}/{im} is not in scene_gt.json / scene_camera.json")
-        for g, v in zip(scenes[s]["gt"][im], scenes[s]["visib"][im]):
+        sc = _scene(scenes, dataset_dir, split, s, im)
+        for g, v in zip(sc["gt"][im], sc["visib"][im]):
             if v >= VISIB_GT_MIN:
                 n_valid[g["obj_id"]] = n_valid.get(g["obj_id"], 0) + 1
     objects = sorted(n_valid)
@@ -544,19 +573,9 @@ def prepare_detection(results, dataset_dir, split="test", targets_name=TARGETS_B
 
 
 def detection_pairs(setup):
-    """Every (kept estimate, ground truth) pair of each group, group after group, each group a row-major [n_est, n_gt]
-    block (the layout gp_bop_match reads).  -> dict of int64 arrays over the pairs: group, est (result index), gt
-    (instance index), frame (index in setup["images"])."""
-    frame = {key: f for f, key in enumerate(setup["images"])}
-    cols = dict(group=[], est=[], gt=[], frame=[])
-    for gi, g in enumerate(setup["groups"]):
-        ne, ng = len(g["est"]), len(g["gt"])
-        if ne and ng:
-            cols["group"].append(np.full(ne * ng, gi))
-            cols["est"].append(np.repeat(np.asarray(g["est"], np.int64), ng))
-            cols["gt"].append(np.tile(np.asarray(g["gt"], np.int64), ne))
-            cols["frame"].append(np.full(ne * ng, frame[(g["scene_id"], g["im_id"])]))
-    return {k: np.concatenate(v).astype(np.int64) if v else np.zeros(0, np.int64) for k, v in cols.items()}
+    """Every (kept estimate, ground truth) pair of every group, laid out as `_pair_rows` says.  -> dict of int64 arrays
+    over the pairs: group, est (result index), gt (instance index), frame (index in setup["images"])."""
+    return _pair_rows(setup["groups"], range(len(setup["groups"])), setup["images"])
 
 
 def _int32p(a):
@@ -589,8 +608,7 @@ def evaluate_detection(results, dataset_dir, split="test", out_dir=None, device=
             raise BopEvalError(f"image {g['scene_id']}/{g['im_id']} has {len(g['gt'])} instances of object "
                                f"{g['obj_id']}, more than {_lib.BOP_MAX_GT_PER_GROUP}")
     oidx = {o: i for i, o in enumerate(objects)}
-    s0, im0 = setup["images"][0]
-    r = image_width(dataset_dir, split, s0, im0) / 640.0
+    r = image_width(dataset_dir, split, *setup["images"][0]) / 640.0
     pairs = detection_pairs(setup)
     n_pairs, n_obj = len(pairs["group"]), len(objects)
     est_off = np.concatenate([[0], np.cumsum([len(g["est"]) for g in groups])]).astype(np.int32)
@@ -601,15 +619,10 @@ def evaluate_detection(results, dataset_dir, split="test", out_dir=None, device=
     lib = _lib.load()
     with torch.cuda.device(device):
         stream = torch.cuda.current_stream(device).cuda_stream
-        mssd = torch.empty(max(n_pairs, 1), device=device)
-        mspd = torch.empty(max(n_pairs, 1), device=device)
+        # one element even for no pairs: gp_bop_match refuses a null pointer, and an empty tensor's data_ptr() is 0
+        mssd = mspd = torch.empty(1, device=device)
         if n_pairs:
-            meshes = [read_ply(os.path.join(setup["mdir"], f"obj_{o:06d}.ply")) for o in objects]
-            vo = np.concatenate([[0], np.cumsum([len(m["vertices"]) for m in meshes])]).astype(np.int32)
-            vertices = torch.as_tensor(np.concatenate([m["vertices"] for m in meshes]), device=device).contiguous()
-            sym = [symmetry_transforms(info[o]) for o in objects]
-            so = np.concatenate([[0], np.cumsum([len(s) for s in sym])]).astype(np.int32)
-            syms = torch.as_tensor(np.concatenate(sym), dtype=torch.float32, device=device).contiguous()
+            _, vertices, syms, vo, so = _object_tables(setup, objects, device)
             K = torch.as_tensor(np.stack([scenes[s]["K"][im] for s, im in setup["images"]]), dtype=torch.float32,
                                 device=device).contiguous()
             pose_of_est = {e: _pose(res[e]["R"], res[e]["t"]) for e in set(rows.tolist())}
@@ -621,16 +634,8 @@ def evaluate_detection(results, dataset_dir, split="test", out_dir=None, device=
             t = lambda a: torch.as_tensor(np.ascontiguousarray(a), device=device)
             obj_d, frame_d = t(pair_obj), t(pairs["frame"].astype(np.int32))
             pe_d, pg_d = t(pose_est), t(pose_gt)
-            vo_c, so_c = (C.c_int32 * len(vo))(*vo.tolist()), (C.c_int32 * len(so))(*so.tolist())
-            done = stages.mark("mssd_mspd")
-            for p0 in range(0, n_pairs, MAX_PAIRS_PER_CALL):
-                n = min(MAX_PAIRS_PER_CALL, n_pairs - p0)
-                check(lib.gp_bop_mssd_mspd(n, n_obj, obj_d[p0:].data_ptr(), vo_c, vertices.data_ptr(), so_c,
-                                           syms.data_ptr(), K.shape[0], K.data_ptr(), frame_d[p0:].data_ptr(),
-                                           pe_d[p0:].data_ptr(), pg_d[p0:].data_ptr(), mssd[p0:].data_ptr(),
-                                           mspd[p0:].data_ptr(), stream))
-            if done is not None:
-                done.record()
+            with stages("mssd_mspd"):
+                mssd, mspd = mssd_mspd(obj_d, vo, vertices, so, syms, K, frame_d, pe_d, pg_d)
         ap = np.zeros((n_obj, 2, T))
         labels = np.zeros((0, 2, T), np.int8)
         if n_rows:
@@ -646,12 +651,10 @@ def evaluate_detection(results, dataset_dir, split="test", out_dir=None, device=
             ws = torch.empty(8 * thr.size + _lib.BOP_MATCH_GROUP_BYTES * len(groups), dtype=torch.uint8, device=device)
             lab_d = torch.empty(n_rows, 2, T, dtype=torch.int8, device=device)
             thr = np.ascontiguousarray(thr)
-            done = stages.mark("match")
-            check(lib.gp_bop_match(len(groups), n_obj, T, _int32p(est_off), _int32p(gt_off), _int32p(group_obj),
-                                   thr.ctypes.data_as(C.POINTER(C.c_double)), mssd.data_ptr(), mspd.data_ptr(),
-                                   valid.data_ptr(), ws.data_ptr(), lab_d.data_ptr(), stream))
-            if done is not None:
-                done.record()
+            with stages("match"):
+                check(lib.gp_bop_match(len(groups), n_obj, T, _int32p(est_off), _int32p(gt_off), _int32p(group_obj),
+                                       thr.ctypes.data_as(C.POINTER(C.c_double)), mssd.data_ptr(), mspd.data_ptr(),
+                                       valid.data_ptr(), ws.data_ptr(), lab_d.data_ptr(), stream))
             # every kept estimate of an object over all images, by descending score, csv order on ties (stable)
             row_obj = np.array([oidx[g["obj_id"]] for g in groups for _ in g["est"]], np.int64)
             score = np.array([res[e]["score"] for e in rows.tolist()], np.float64)
@@ -661,12 +664,10 @@ def evaluate_detection(results, dataset_dir, split="test", out_dir=None, device=
             rec = np.ascontiguousarray(RECALL_THRESHOLDS, np.float64)
             rank_d = torch.as_tensor(order, device=device)
             ap_d = torch.empty(n_obj, 2, T, dtype=torch.float64, device=device)
-            done = stages.mark("ap")
-            check(lib.gp_bop_average_precision(n_obj, T, n_rows, lab_d.data_ptr(), _int32p(rank_off), rank_d.data_ptr(),
-                                               _int32p(nv), len(rec), rec.ctypes.data_as(C.POINTER(C.c_double)),
-                                               ap_d.data_ptr(), stream))
-            if done is not None:
-                done.record()
+            with stages("ap"):
+                check(lib.gp_bop_average_precision(n_obj, T, n_rows, lab_d.data_ptr(), _int32p(rank_off),
+                                                   rank_d.data_ptr(), _int32p(nv), len(rec),
+                                                   rec.ctypes.data_as(C.POINTER(C.c_double)), ap_d.data_ptr(), stream))
             ap, labels = ap_d.cpu().numpy(), lab_d.cpu().numpy()
         errors = dict(group=pairs["group"], est=pairs["est"], gt=pairs["gt"], mssd=mssd[:n_pairs].cpu().numpy(),
                       mspd=mspd[:n_pairs].cpu().numpy())
@@ -677,12 +678,9 @@ def evaluate_detection(results, dataset_dir, split="test", out_dir=None, device=
     out = dict(map=(map_mssd + map_mspd) / 2.0, map_mssd=map_mssd, map_mspd=map_mspd, ap_mssd=ap_mssd, ap_mspd=ap_mspd,
                objects=list(objects), average_time_per_image=average_time_per_image(res), errors=errors,
                labels=labels, rows=rows)
-    if out_dir is not None:
-        os.makedirs(out_dir, exist_ok=True)
-        scores = {"bop24_mAP": out["map"], "bop24_mAP_mssd": map_mssd, "bop24_mAP_mspd": map_mspd,
-                  "bop24_average_time_per_image": out["average_time_per_image"]}
-        with open(os.path.join(out_dir, "scores_bop24.json"), "w") as f:
-            json.dump(scores, f, indent=2)
+    _write_scores(out_dir, "scores_bop24.json", {"bop24_mAP": out["map"], "bop24_mAP_mssd": map_mssd,
+                                                 "bop24_mAP_mspd": map_mspd,
+                                                 "bop24_average_time_per_image": out["average_time_per_image"]})
     return out
 
 

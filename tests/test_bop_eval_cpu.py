@@ -71,6 +71,15 @@ def test_a_dataset_without_depth_is_refused(tmp_path):
         bop_eval.load_depth(str(tmp_path), "test", 1, 0, 1.0)
 
 
+def test_a_targets_file_without_targets_is_refused(tmp_path):
+    """Refused while reading the dataset, before any device work: there is nothing to score."""
+    _tree(tmp_path)
+    with open(tmp_path / "test_targets_bop19.json", "w") as f:
+        json.dump([], f)
+    with pytest.raises(bop_eval.BopEvalError, match="lists no targets"):
+        bop_eval.evaluate([], str(tmp_path), device="cuda:0")
+
+
 def test_symmetry_counts_fixed_axis_and_composition_order():
     n = int(np.ceil(np.pi / 0.01))
     assert n == 315
