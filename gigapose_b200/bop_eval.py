@@ -62,13 +62,20 @@ def load_scene(dataset_dir, split, scene_id):
     d = os.path.join(dataset_dir, split, f"{scene_id:06d}")
     gt = _json(os.path.join(d, "scene_gt.json"))
     info = _json(os.path.join(d, "scene_gt_info.json"))
-    cam = _json(os.path.join(d, "scene_camera.json"))
-    out = dict(gt={}, visib={}, K={}, depth_scale={})
+    out = dict(gt={}, visib={}, **load_cameras(dataset_dir, split, scene_id))
     for im, insts in gt.items():
         out["gt"][int(im)] = [dict(R=np.asarray(g["cam_R_m2c"], np.float64).reshape(3, 3),
                                    t=np.asarray(g["cam_t_m2c"], np.float64).reshape(3), obj_id=int(g["obj_id"]))
                               for g in insts]
         out["visib"][int(im)] = [float(i["visib_fract"]) for i in info[im]]
+    return out
+
+
+def load_cameras(dataset_dir, split, scene_id):
+    """-> dict(K={im: [3,3]}, depth_scale={im: float}) from a scene's scene_camera.json (test splits without ground
+    truth, such as those of hb and itodd, have this file only)."""
+    cam = _json(os.path.join(dataset_dir, split, f"{scene_id:06d}", "scene_camera.json"))
+    out = dict(K={}, depth_scale={})
     for im, c in cam.items():
         out["K"][int(im)] = np.asarray(c["cam_K"], np.float64).reshape(3, 3)
         out["depth_scale"][int(im)] = float(c.get("depth_scale", 1.0))

@@ -1,0 +1,447 @@
+"""Row f9: GigaPose on a BOP test split, from the dataset directory and its default CNOS detections to the results csv
+(and, with --evaluate, to scores_bop19.json / scores_bop24.json) -- the reference's `test.py` with its test dataloader
+(dataloader/test.py, utils/inout.py:370-492) and Lightning loop, without Hydra, Lightning, webdataset or the BOP toolkit.
+
+Each image is one step, as in test.py:55-60: its CNOS masks stay COCO run-length encodings and are cropped on the GPU
+(`preprocess.crop_detections_rle`, gp_crop_resize_pad_rle), then `GigaPose.eval_retrieval` writes the step's
+predictions/{idx}.npz, and `save_predictions_from_batched_predictions` writes the csv at the end.  A background thread
+decodes the next image into pinned memory while the current one runs.  INTEGRATION.md lists every deviation from
+test.py.  Usage:
+
+    python -m gigapose_b200.bop_run --dataset-dir D --checkpoint gigaPose_v1.ckpt --template-poses P.npy
+        [--setting localization|detection] [--detections FILE] [--out DIR] [--evaluate]
+"""
+from __future__ import annotations
+
+import argparse
+import concurrent.futures
+import copy
+import glob
+import json
+import os
+import pickle
+import types
+
+import numpy as np
+import torch
+
+from .bop_eval import load_cameras
+
+CAP_PER_TARGET = 16             # localization: detections kept per target (dataloader/test.py:110-114)
+CAP_PER_TARGET_ICBIN = 32
+LMO_INDEX_TO_ID = [1, 5, 6, 8, 9, 10, 11, 12]      # src/utils/dataset.py: the LM-O labels the model is indexed with
+LMO_ID_TO_INDEX = {o: i + 1 for i, o in enumerate(LMO_INDEX_TO_ID)}
+
+
+class BopRunError(ValueError):
+    pass
+
+
+# ---------------------------------------------------------------------------------------------------- dataset layout
+def split_name(dataset_name):
+    """(split, model directory) of a dataset's test images (`get_split_name`, dataloader/test.py:155-165)."""
+    split = "test_primesense" if dataset_name in ("hb", "tless") else "test"
+    return split, "models_cad" if dataset_name == "tless" else "models"
+
+
+def detection_year(dataset_name):
+    """(BOP year, CNOS variant) of the default detections (utils/inout.py:408-417)."""
+    if dataset_name in ("lmo", "tless", "tudl", "icbin", "itodd", "hb", "ycbv"):
+        return "19", "cnos-fastsam"
+    if dataset_name == "hope":
+        return "24", "cnos-sam"
+    raise BopRunError(f"dataset {dataset_name!r} has no default detections; pass --detections")
+
+
+def default_detections(dataset_dir):
+    """<parent of dataset_dir>/default_detections/core{19,24}_model_based_unseen/cnos-*/ : the first file (by name)
+    whose name contains the dataset name (utils/inout.py:418-424, which takes the first in directory order)."""
+    name = os.path.basename(os.path.normpath(dataset_dir))
+    year, model = detection_year(name)
+    d = os.path.join(os.path.dirname(os.path.abspath(dataset_dir)), "default_detections",
+                     f"core{year}_model_based_unseen", model)
+    found = sorted(f for f in os.listdir(d) if name in f) if os.path.isdir(d) else []
+    if not found:
+        raise BopRunError(f"no detection file for {name!r} in {d}")
+    return os.path.join(d, found[0])
+
+
+def image_path(dataset_dir, split, scene_id, im_id):
+    """rgb/*.jpg, else rgb/*.png, else gray/*.tif (web_scene_dataset.py:38-45)."""
+    d = os.path.join(dataset_dir, split, f"{scene_id:06d}")
+    for sub, ext in (("rgb", "jpg"), ("rgb", "png"), ("gray", "tif")):
+        p = os.path.join(d, sub, f"{im_id:06d}.{ext}")
+        if os.path.exists(p):
+            return p
+    raise BopRunError(f"no image {im_id:06d}.jpg/.png under {d}/rgb nor .tif under {d}/gray")
+
+
+def read_image(path):
+    """-> u8 [H,W,3] as decoded; a gray image is repeated to three channels.  Refuses anything but 8-bit data."""
+    from PIL import Image
+    with Image.open(path) as im:
+        a = np.asarray(im)
+    if a.dtype != np.uint8:
+        raise BopRunError(f"{path} holds {a.dtype} pixels; only 8-bit images are supported")
+    if a.ndim == 2:
+        a = np.stack([a, a, a], axis=-1)
+    if a.ndim != 3 or a.shape[2] != 3:
+        raise BopRunError(f"{path} has shape {a.shape}; expected [H,W] gray or [H,W,3] RGB")
+    return a
+
+
+# ---------------------------------------------------------------------------------------------------- RLE
+def rle_from_string(s):
+    """COCO's compressed RLE string (`rleFrString` of the COCO mask API) -> list of run lengths."""
+    counts, p = [], 0
+    data = s.encode() if isinstance(s, str) else bytes(s)
+    while p < len(data):
+        x, k, more = 0, 0, True
+        while more:
+            if p >= len(data):
+                raise BopRunError("truncated compressed RLE string")
+            c = data[p] - 48
+            if not 0 <= c < 64:
+                raise BopRunError(f"byte {data[p]!r} is not a compressed RLE character")
+            x |= (c & 0x1F) << (5 * k)
+            more = bool(c & 0x20)
+            p += 1
+            k += 1
+            if not more and (c & 0x10):
+                x |= -1 << (5 * k)
+        if len(counts) > 2:
+            x += counts[-2]
+        counts.append(x)
+    return counts
+
+
+def rle_counts(segmentation, shape, where):
+    """A detection's `segmentation` (dict(size [H, W], counts: list or compressed string)) -> i32 run lengths, after
+    checking that its size is the image's (H, W) and that no run is negative; `where` names the detection in errors."""
+    size = [int(v) for v in segmentation.get("size", ())]
+    if size != list(shape):
+        raise BopRunError(f"{where}: mask size {size} differs from the image's {list(shape)}")
+    c = segmentation.get("counts")
+    if isinstance(c, (str, bytes)):
+        c = rle_from_string(c)
+    c = np.asarray(c, np.int64).reshape(-1)
+    if c.size and c.min() < 0:
+        raise BopRunError(f"{where}: negative run length {int(c.min())}")
+    if c.size and c.max() > np.iinfo(np.int32).max:
+        raise BopRunError(f"{where}: run length {int(c.max())} does not fit 32 bits")
+    return c.astype(np.int32)
+
+
+# ---------------------------------------------------------------------------------------------------- detections
+def _key(scene_id, im_id):
+    return f"{int(scene_id):06d}_{int(im_id):06d}"
+
+
+def _by_image(dets, image_key):
+    """`group_by_image_level` (utils/inout.py:109-123): {"scene_im": [det]} in order of first appearance."""
+    out = {}
+    for d in dets:
+        out.setdefault(_key(d["scene_id"], d[image_key]), []).append(d)
+    return out
+
+
+def select_detections(dets, dataset_name, setting, targets=None):
+    """`load_test_list_and_cnos_detections` + `generate_test_list` (utils/inout.py:370-492) with the caps of
+    `GigaPoseTestSet.load_detections` (dataloader/test.py:110-114).  dets: the CNOS list; targets: the
+    test_targets_bop*.json list (localization).  -> (test_list {key: [dict(scene_id, im_id, obj_id, inst_count)]},
+    detections {key: [det]}).  Localization: per target, its object's detections of the image (all of the image's,
+    relabelled, when it has none), by descending score (stable), at most 16 (32 for icbin); detection: every detection
+    of each image, one target per object with its count.  The detections are deep copies of the input's."""
+    per_image = _by_image(dets, "image_id")
+    if setting == "detection":
+        test_list = {}
+        for key, im_dets in per_image.items():
+            counts = {}
+            for d in im_dets:
+                counts[d["category_id"]] = counts.get(d["category_id"], 0) + 1
+            s, im = (int(v) for v in key.split("_"))
+            test_list[key] = [dict(scene_id=s, im_id=im, obj_id=o, inst_count=n) for o, n in counts.items()]
+        return test_list, {k: copy.deepcopy(v) for k, v in per_image.items()}
+    if setting != "localization":
+        raise BopRunError(f"setting {setting!r} is neither 'localization' nor 'detection'")
+    if targets is None:
+        raise BopRunError("the localization setting needs the test targets")
+    cap = CAP_PER_TARGET_ICBIN if dataset_name == "icbin" else CAP_PER_TARGET
+    selected = []
+    for t in targets:
+        key = _key(t["scene_id"], t["im_id"])
+        if key not in per_image:
+            raise BopRunError(f"target image {key} (object {t['obj_id']}) has no detection")
+        chosen = [d for d in per_image[key] if d["category_id"] == t["obj_id"]]
+        if not chosen:                                   # MegaPose's fallback: every detection of the image
+            chosen = copy.deepcopy(per_image[key])
+            for d in chosen:
+                d["category_id"] = t["obj_id"]
+        chosen = sorted(chosen, key=lambda d: d["score"], reverse=True)[:cap]
+        selected.extend(copy.deepcopy(chosen))
+    return _by_image(targets, "im_id"), _by_image(selected, "image_id")
+
+
+def xywh_to_xyxy(bbox):
+    """CNOS xywh -> i64 xyxy as the reference's collate makes it: float32 x, y, x + w, y + h truncated toward zero
+    (scene_dataset.py:337, bbox.py:6-22,116-130)."""
+    b = np.asarray(bbox, np.float32).reshape(-1, 4)
+    return np.stack([b[:, 0], b[:, 1], b[:, 0] + b[:, 2], b[:, 1] + b[:, 3]], 1).astype(np.int64)
+
+
+def image_inputs(dets, targets, dataset_name, shape, key):
+    """One image's host inputs: labels (object ids, LM-O indices for lmo), i64 xyxy boxes, concatenated i32 RLE counts
+    and their offsets [n+1], the test list rows and the image's detection time (its first detection's)."""
+    remap = (lambda o: LMO_ID_TO_INDEX[int(o)]) if "lmo" in dataset_name else int
+    counts = [rle_counts(d["segmentation"], shape, f"image {key}, detection {i}") for i, d in enumerate(dets)]
+    return dict(labels=np.array([remap(d["category_id"]) for d in dets], np.int64),
+                boxes=xywh_to_xyxy([d["bbox"] for d in dets]),
+                counts=np.concatenate(counts) if counts else np.zeros(0, np.int32),
+                offsets=np.concatenate([[0], np.cumsum([len(c) for c in counts])]).astype(np.int64),
+                obj_id=[remap(t["obj_id"]) for t in targets], inst_count=[int(t["inst_count"]) for t in targets],
+                detection_time=float(dets[0].get("time", 0.0)))
+
+
+# ---------------------------------------------------------------------------------------------------- model
+_SAFE_BUILTINS = {"set", "frozenset", "slice", "range", "complex", "bytearray", "list", "dict", "tuple", "int", "float",
+                  "bool", "str", "bytes", "object"}
+
+
+class _Inert:
+    """Stands in for a pickled class this process does not have (Hydra / omegaconf hyper-parameters): it takes any
+    arguments and state and does nothing."""
+
+    def __init__(self, *args, **kwargs):
+        pass
+
+    def __setstate__(self, state):
+        self.__dict__["_state"] = state
+
+
+class _Unpickler(pickle.Unpickler):
+    """Resolves torch, numpy, collections and plain builtin types; every other class becomes an `_Inert` subclass of
+    the same name, so unpickling runs no code from other modules."""
+
+    def find_class(self, module, name):
+        root = module.split(".")[0]
+        if root in ("torch", "numpy", "collections", "_codecs") or (module == "builtins" and name in _SAFE_BUILTINS) \
+                or (module == "copyreg" and name == "_reconstructor"):
+            try:
+                return super().find_class(module, name)
+            except (ImportError, AttributeError):
+                pass
+        return type(name, (_Inert,), {"__module__": module})
+
+
+_pickle = types.ModuleType("gigapose_b200_checkpoint_pickle")
+_pickle.Unpickler = _Unpickler
+_pickle.load = lambda f, **kw: _Unpickler(f, **kw).load()
+
+
+def load_state_dict(path):
+    """The `state_dict` of a Lightning checkpoint (tensors on the CPU); its other entries are unpickled inertly."""
+    ckpt = torch.load(path, map_location="cpu", pickle_module=_pickle, weights_only=False)
+    if not isinstance(ckpt, dict) or not isinstance(ckpt.get("state_dict"), dict):
+        raise BopRunError(f"{path} has no state_dict (not a Lightning checkpoint)")
+    return ckpt["state_dict"]
+
+
+def load_checkpoint(model, path):
+    """Loads a Lightning checkpoint's state_dict into `model` strictly; a missing or unexpected key is named."""
+    state = load_state_dict(path)
+    own = set(model.state_dict())
+    missing, unexpected = sorted(own - set(state)), sorted(set(state) - own)
+    if missing or unexpected:
+        raise BopRunError(f"{path} does not fit the model: missing keys {missing}, unexpected keys {unexpected}")
+    model.load_state_dict(state, strict=True)
+    return model
+
+
+def build_model(device, log_dir, checkpoint=None, seed=None):
+    """The `GigaPose` of configs/model/large.yaml (DINOv2 ViT-L/14 descriptors, ResNet IST trunk, k = 5), built in code
+    as bench.build_models builds it.  With `checkpoint`, its state_dict is loaded strictly (a missing or unexpected
+    key is named); `seed` seeds the initial weights (tests), otherwise they are the constructors' defaults."""
+    from gigapose_b200.vit import DinoVisionTransformer
+    from src.models.gigaPose import GigaPose
+    from src.models.matching import LocalSimilarity
+    from src.models.network.ae_net import AENet
+    from src.models.network.ist_net import ISTNet, Regressor
+    from src.models.network.resnet import ResNet
+
+    vit = DinoVisionTransformer(init_seed=seed)
+    ae = AENet("dinov2_vitl14", dinov2_model=vit, descriptor_size=1024, max_batch_size=64)
+    if seed is not None:
+        torch.manual_seed(seed + 1)
+    backbone = ResNet(dict(n_heads=0, input_dim=3, input_size=256, initial_dim=128, block_dims=[128, 192, 256, 512],
+                           descriptor_size=256))
+    reg = Regressor(descriptor_size=256, hidden_dim=256, use_tanh_act=True, normalize_output=True)
+    ist = ISTNet("resnet", backbone, reg, max_batch_size=64)
+    metric = LocalSimilarity(k=5, sim_threshold=0.5, patch_threshold=3)
+    model = GigaPose("large", ae, ist, training_loss=None, testing_metric=metric, optim_config=None, log_interval=1000,
+                     log_dir=log_dir, max_num_dets_per_forward=None)
+    if checkpoint is not None:
+        load_checkpoint(model, checkpoint)
+    return model.to(device).eval()
+
+
+def object_ids(dataset_dir, dataset_name):
+    """Object ids in the model's label order (label i is object_ids[i - 1]): the LM-O order for lmo, else 1 .. N."""
+    _, mname = split_name(dataset_name)
+    with open(os.path.join(dataset_dir, mname, "models_info.json")) as f:
+        ids = sorted(int(k) for k in json.load(f))
+    if "lmo" in dataset_name:
+        if sorted(LMO_INDEX_TO_ID) != ids:
+            raise BopRunError(f"lmo models_info.json lists objects {ids}, not {LMO_INDEX_TO_ID}")
+        return list(LMO_INDEX_TO_ID)
+    if ids != list(range(1, len(ids) + 1)):
+        raise BopRunError(f"object ids {ids} are not 1 .. {len(ids)}: labels index the template bank")
+    return ids
+
+
+def onboard(model, dataset_dir, template_poses, dataset_name=None):
+    """`GigaPose.onboard_meshes` on the dataset's meshes (models/ or models_cad/, object_ids order) with the [T,4,4]
+    template poses of INTEGRATION.md (an .npy path or an array)."""
+    from gigapose_b200.render import read_ply
+    name = dataset_name or os.path.basename(os.path.normpath(dataset_dir))
+    _, mname = split_name(name)
+    poses = np.load(template_poses) if isinstance(template_poses, (str, os.PathLike)) else np.asarray(template_poses)
+    if poses.ndim != 3 or poses.shape[1:] != (4, 4):
+        raise BopRunError(f"template poses must be [T,4,4], got {poses.shape}")
+    meshes = [read_ply(os.path.join(dataset_dir, mname, f"obj_{o:06d}.ply")) for o in object_ids(dataset_dir, name)]
+    return model.onboard_meshes(name, meshes, torch.as_tensor(poses, dtype=torch.float32))
+
+
+# ---------------------------------------------------------------------------------------------------- the loop
+def plan(dataset_dir, setting="localization", detections=None, dataset_name=None):
+    """Everything the loop needs from the host: dict(name, split, images [(scene, im)] in sorted order, test_list,
+    detections, cameras {scene: {im: K}})."""
+    name = dataset_name or os.path.basename(os.path.normpath(dataset_dir))
+    split, _ = split_name(name)
+    path = detections or default_detections(dataset_dir)
+    with open(path) as f:
+        dets = json.load(f)
+    targets = None
+    if setting == "localization":
+        year = "24" if name == "hope" else "19"
+        tpath = os.path.join(dataset_dir, f"test_targets_bop{year}.json")
+        if not os.path.exists(tpath):
+            raise BopRunError(f"{tpath} not found: the localization setting needs the test targets")
+        with open(tpath) as f:
+            targets = json.load(f)
+    test_list, selected = select_detections(dets, name, setting, targets)
+    images = sorted({tuple(int(v) for v in k.split("_")) for k in test_list})
+    cams = {}
+    for s in sorted({s for s, _ in images}):
+        cams[s] = load_cameras(dataset_dir, split, s)["K"]
+    for s, im in images:
+        if im not in cams[s]:
+            raise BopRunError(f"image {_key(s, im)} is not in scene_camera.json")
+    return dict(name=name, split=split, images=images, test_list=test_list, detections=selected, cameras=cams,
+                dataset_dir=dataset_dir)
+
+
+class _Prefetch:
+    """Decodes image i + 1 on a background thread into one of two pinned buffers while image i runs."""
+
+    def __init__(self, paths):
+        self.paths, self.pool, self.bufs = paths, concurrent.futures.ThreadPoolExecutor(1), {}
+        self.next = self.pool.submit(self._load, 0) if paths else None
+
+    def _load(self, i):
+        a = read_image(self.paths[i])
+        key = (i % 2, a.shape)
+        buf = self.bufs.get(key)
+        if buf is None:
+            buf = self.bufs[key] = torch.empty(a.shape, dtype=torch.uint8, pin_memory=True)
+        buf.numpy()[...] = a
+        return buf
+
+    def get(self, i):
+        buf = self.next.result()
+        self.next = self.pool.submit(self._load, i + 1) if i + 1 < len(self.paths) else None
+        return buf
+
+    def close(self):
+        self.pool.shutdown(wait=True)
+
+
+def image_batch(p, i, rgb, device):
+    """Step i's batch for `eval_retrieval`: the RLE crop of the image's detections on the device plus the infos and
+    test list the reference's collate builds (dataloader/test.py:167-205, 283-293)."""
+    import pandas as pd
+    import src.megapose.utils.tensor_collection as tc
+    from .preprocess import crop_detections_rle
+    s, im = p["images"][i]
+    key = _key(s, im)
+    x = image_inputs(p["detections"][key], p["test_list"][key], p["name"], tuple(rgb.shape[:2]), key)
+    n = len(x["labels"])
+    crop = crop_detections_rle(rgb.to(device, non_blocking=True)[None], x["counts"], x["offsets"], x["boxes"],
+                               np.zeros(n, np.int64))
+    K = torch.as_tensor(p["cameras"][s][im], dtype=torch.float64).float().to(device).expand(n, 3, 3).contiguous()
+    infos = pd.DataFrame(dict(label=[str(v) for v in x["labels"]], scene_id=[s] * n, view_id=[im] * n,
+                              batch_im_id=np.zeros(n, np.int64)))
+    batch = tc.PandasTensorCollection(infos=infos, tar_img=crop["tar_img"], tar_mask=crop["tar_mask"], tar_K=K,
+                                      tar_M=crop["tar_M"])
+    batch.test_list = tc.PandasTensorCollection(infos=pd.DataFrame(dict(
+        im_id=[im] * len(x["obj_id"]), scene_id=[s] * len(x["obj_id"]), obj_id=x["obj_id"],
+        inst_count=x["inst_count"], detection_time=[x["detection_time"]] * len(x["obj_id"]))))
+    return batch
+
+
+@torch.no_grad()
+def run(model, dataset_dir, out_dir, setting="localization", detections=None, template_poses=None, run_id="bop_run",
+        dataset_name=None):
+    """Runs the test split: onboards the dataset from `template_poses` unless the model already holds it, then one
+    `eval_retrieval` per image (predictions under out_dir/predictions, which must hold no .npz yet) and the csv.
+    -> path of the csv (`{model}-pbrreal-rgb-mmodel_{dataset}-test_{run_id}.csv` in out_dir/predictions)."""
+    from src.utils.inout import save_predictions_from_batched_predictions
+    p = plan(dataset_dir, setting, detections, dataset_name)
+    pred_dir = os.path.join(out_dir, "predictions")
+    os.makedirs(pred_dir, exist_ok=True)
+    if glob.glob(os.path.join(glob.escape(pred_dir), "*.npz")):
+        raise BopRunError(f"{pred_dir} already holds prediction files; use an empty --out")
+    if p["name"] not in model.engines:
+        if template_poses is None:
+            raise BopRunError(f"{p['name']} is not onboarded and no template poses were given")
+        onboard(model, dataset_dir, template_poses, p["name"])
+    model.log_dir = out_dir
+    device = model.engines[p["name"]].device
+    pre = _Prefetch([image_path(dataset_dir, p["split"], s, im) for s, im in p["images"]])
+    try:
+        for i in range(len(p["images"])):
+            batch = image_batch(p, i, pre.get(i), device)
+            model.eval_retrieval(batch, idx_batch=i, dataset_name=p["name"])
+    finally:
+        pre.close()
+    save_predictions_from_batched_predictions(pred_dir, dataset_name=p["name"], model_name=model.model_name,
+                                              run_id=run_id, is_refined=False)
+    return os.path.join(pred_dir, f"{model.model_name}-pbrreal-rgb-mmodel_{p['name']}-test_{run_id}.csv")
+
+
+def main(argv=None):
+    ap = argparse.ArgumentParser(description="GigaPose on a BOP test split with its CNOS detections -> BOP results csv")
+    ap.add_argument("--dataset-dir", required=True, help="BOP dataset directory, e.g. <root>/lmo")
+    ap.add_argument("--checkpoint", required=True, help="Lightning checkpoint (gigaPose_v1.ckpt)")
+    ap.add_argument("--template-poses", required=True, help="[T,4,4] .npy of template poses (see INTEGRATION.md)")
+    ap.add_argument("--setting", choices=("localization", "detection"), default="localization")
+    ap.add_argument("--detections", default=None, help="CNOS detections json (default: <root>/default_detections/...)")
+    ap.add_argument("--out", default="bop_run_out")
+    ap.add_argument("--evaluate", action="store_true", help="score the csv with bop_eval")
+    ap.add_argument("--device", default="cuda")
+    a = ap.parse_args(argv)
+    model = build_model(a.device, a.out, checkpoint=a.checkpoint)
+    csv = run(model, a.dataset_dir, a.out, a.setting, a.detections, a.template_poses)
+    print(csv)
+    if a.evaluate:
+        from . import bop_eval
+        split, _ = split_name(os.path.basename(os.path.normpath(a.dataset_dir)))
+        if a.setting == "localization":
+            res = bop_eval.evaluate(csv, a.dataset_dir, split, out_dir=a.out, device=a.device)
+            print(json.dumps({k: res[k] for k in ("ar", "ar_vsd", "ar_mssd", "ar_mspd", "n_targets")}))
+        else:
+            res = bop_eval.evaluate_detection(csv, a.dataset_dir, split, out_dir=a.out, device=a.device)
+            print(json.dumps({k: res[k] for k in ("map", "map_mssd", "map_mspd")}))
+
+
+if __name__ == "__main__":
+    main()

@@ -4,8 +4,10 @@ src/utils/crop.py:16-61) as one gather kernel, optionally fused with the dataloa
 """
 from __future__ import annotations
 
+import ctypes as C
 from typing import Optional, Sequence
 
+import numpy as np
 import torch
 
 from . import _lib
@@ -66,3 +68,42 @@ def preprocess_queries(rgb_u8: torch.Tensor, masks: torch.Tensor, xyxy_boxes: to
     r = crop_resize_pad(xyxy_boxes, rgb_u8.to(torch.float32), target_size, image_index=batch_im_id, mask=masks, in_div=255.0,
                         mean=CLIP_MEAN, std=CLIP_STD)
     return {"tar_img": r["images"], "tar_mask": r["mask"], "tar_M": r["M"]}
+
+
+@torch.no_grad()
+def crop_detections_rle(rgb_hwc: torch.Tensor, counts, offsets, xyxy_boxes, batch_im_id, target_size: int = 224):
+    """`preprocess_queries` for masks given as COCO run-length encodings (row f9, gp_crop_resize_pad_rle): the dense
+    masks are never built.  rgb_hwc u8 [m,H,W,3] on a CUDA device, counts i32 [sum of runs] (every detection's runs,
+    concatenated; host or device), offsets [n+1] host ints (detection i owns counts[offsets[i]:offsets[i+1]]), boxes
+    [n,4] xyxy, batch_im_id [n] -> tar_img [n,3,T,T], tar_mask [n,T,T], tar_M [n,3,3], bit for bit those of
+    `preprocess_queries` on the decoded masks."""
+    if not rgb_hwc.is_cuda:
+        raise _lib.GigaPoseNativeError("crop_detections_rle runs on CUDA tensors only (no CPU fallback)")
+    if rgb_hwc.dtype != torch.uint8 or rgb_hwc.dim() != 4 or rgb_hwc.shape[-1] != 3:
+        raise ValueError(f"rgb_hwc must be uint8 [m,H,W,3], got {rgb_hwc.dtype} {tuple(rgb_hwc.shape)}")
+    lib = _lib.load()
+    dev = rgb_hwc.device
+    images = rgb_hwc.contiguous()
+    m, H, W, _ = images.shape
+    boxes = torch.as_tensor(xyxy_boxes, device=dev).long().contiguous()
+    n = boxes.shape[0]
+    idx = torch.as_tensor(batch_im_id).to(torch.int64)
+    if idx.shape != (n,) or (n and (int(idx.min()) < 0 or int(idx.max()) >= m)):
+        raise ValueError(f"batch_im_id must be [{n}] indices into {m} images")
+    idx = idx.to(device=dev, dtype=torch.int32, non_blocking=True)
+    off = np.ascontiguousarray(np.asarray(offsets, np.int64).reshape(-1))
+    if off.shape != (n + 1,):
+        raise ValueError(f"offsets must have n + 1 = {n + 1} entries, got {off.shape[0]}")
+    cnt = torch.as_tensor(counts, dtype=torch.int32).to(dev, non_blocking=True).contiguous()
+    if cnt.numel() < off[-1]:
+        raise ValueError(f"offsets end at {off[-1]} but counts holds {cnt.numel()} runs")
+    ends = torch.empty(max(int(off[-1]), 1), dtype=torch.int64, device=dev)
+    T = int(target_size)
+    out = torch.empty(n, 3, T, T, device=dev)
+    out_mask = torch.empty(n, T, T, device=dev)
+    M = torch.empty(n, 3, 3, device=dev)
+    with torch.cuda.device(dev):
+        check(lib.gp_crop_resize_pad_rle(n, H, W, T, images.data_ptr(), idx.data_ptr(), boxes.data_ptr(), ptr(cnt),
+                                         off.ctypes.data_as(C.POINTER(C.c_int64)), ends.data_ptr(), out.data_ptr(),
+                                         out_mask.data_ptr(), M.data_ptr(), torch.cuda.current_stream(dev).cuda_stream))
+    return {"tar_img": out, "tar_mask": out_mask, "tar_M": M}

@@ -271,6 +271,19 @@ int gp_crop_resize_pad(int n, int channels, int height, int width, int target_si
                        const int32_t* image_index, const int64_t* xyxy_boxes, const float* mask, float in_div,
                        const float* post_sub, const float* post_div, float* out_images, float* out_mask, float* out_M,
                        void* stream);
+/* Row f9: the same crop for CNOS detections whose masks are COCO run-length encodings, in place of the dense
+ * `pycoco_utils.rle_to_binary_mask` masks of the reference's test loader (dataloader/test.py:238, train.py:82,107-110,
+ * transform.yaml:2-7).  Outputs are those of gp_crop_resize_pad with channels = 3, the mask, in_div = 255 and the CLIP
+ * mean / std, bit for bit.  images u8 [*,H,W,3] (HWC, as decoded), image_index i32 [n] (device); detection i's runs are
+ * counts[offsets[i] .. offsets[i+1]) (i32, device): column-major (pixel (row, col) is run position col * H + row), the
+ * first run counts zeros, runs alternate, anything past the last run is 0 and runs past H * W are cut off.  offsets
+ * i64 [n+1] is HOST memory, non-decreasing from offsets[0] >= 0; ends i64 (device, offsets[n] elements) is scratch that
+ * receives each detection's running sums.  out_images f32 [n,3,T,T], out_mask f32 [n,T,T], out_M f32 [n,3,3].  Two
+ * launches per 256 detections.  Needs no handle. */
+int gp_crop_resize_pad_rle(int n, int height, int width, int target_size, const uint8_t* images,
+                           const int32_t* image_index, const int64_t* xyxy_boxes, const int32_t* counts,
+                           const int64_t* offsets, int64_t* ends, float* out_images, float* out_mask, float* out_M,
+                           void* stream);
 
 /* --- row f5: template renders from a CAD mesh (the Panda3D call of src/custom_megapose/call_panda3d.py:45-59 plus the
  * PNG round trip and bounding box of custom_megapose/template_dataset.py:66-119).  The full contract is the header
