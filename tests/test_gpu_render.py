@@ -9,46 +9,14 @@ import torch
 
 from gigapose_b200 import render, synth
 from oracle import render_port as rp
+from render_fp64 import icosphere
+from render_fp64 import uv_sphere as _uv_sphere
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
 K_FULL = np.array(render.TEMPLATE_K, np.float32)
 K_QUARTER = np.array([[K_FULL[0, 0] / 4, 0, K_FULL[0, 2] / 4], [0, K_FULL[1, 1] / 4, K_FULL[1, 2] / 4], [0, 0, 1]],
                      np.float32)
-
-
-def icosphere(subdiv, radius, rng, bumps=0.15):
-    t = (1 + 5 ** 0.5) / 2
-    V = [[-1, t, 0], [1, t, 0], [-1, -t, 0], [1, -t, 0], [0, -1, t], [0, 1, t], [0, -1, -t], [0, 1, -t],
-         [t, 0, -1], [t, 0, 1], [-t, 0, -1], [-t, 0, 1]]
-    Fc = [[0, 11, 5], [0, 5, 1], [0, 1, 7], [0, 7, 10], [0, 10, 11], [1, 5, 9], [5, 11, 4], [11, 10, 2], [10, 7, 6],
-          [7, 1, 8], [3, 9, 4], [3, 4, 2], [3, 2, 6], [3, 6, 8], [3, 8, 9], [4, 9, 5], [2, 4, 11], [6, 2, 10],
-          [8, 6, 7], [9, 8, 1]]
-    V = [np.array(v, float) / np.linalg.norm(v) for v in V]
-    for _ in range(subdiv):
-        mid, out = {}, []
-
-        def m(a, b):
-            key = (min(a, b), max(a, b))
-            if key not in mid:
-                p = V[a] + V[b]
-                V.append(p / np.linalg.norm(p))
-                mid[key] = len(V) - 1
-            return mid[key]
-        for a, b, c in Fc:
-            ab, bc, ca = m(a, b), m(b, c), m(c, a)
-            out += [[a, ab, ca], [b, bc, ab], [c, ca, bc], [ab, bc, ca]]
-        Fc = out
-    V = np.array(V)
-    V *= radius * (1 + bumps * rng.uniform(-1, 1, (len(V), 1)))
-    return V.astype(np.float32), np.array(Fc, np.int32)
-
-
-def _uv_sphere(V, Fc, scale):
-    """Per-corner UVs from longitude / latitude, scaled past [0, 1] so that the repeat wrap is exercised."""
-    d = V / np.linalg.norm(V, axis=1, keepdims=True)
-    uv = np.stack([np.arctan2(d[:, 1], d[:, 0]) / (2 * np.pi) + 0.5, np.arccos(np.clip(d[:, 2], -1, 1)) / np.pi], 1)
-    return (uv[Fc] * scale).astype(np.float32)
 
 
 def meshes():
