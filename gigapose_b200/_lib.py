@@ -162,6 +162,8 @@ SYMBOLS = {
                                 C.c_void_p, C.c_void_p, C.POINTER(GpIcpParams), C.c_void_p, C.c_void_p, C.c_void_p,
                                 C.c_void_p, C.c_void_p, C.c_void_p]),
     "gp_debug_icp_select": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
+    "gp_depth_score": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
+                                 C.c_void_p, C.c_float, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "gp_ist_trunk_query_sizes":(C.c_int, [C.c_int, C.POINTER(C.c_size_t), C.POINTER(C.c_size_t)]),
     "gp_ist_trunk_create": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                       C.POINTER(C.c_void_p)]),

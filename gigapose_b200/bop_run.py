@@ -6,10 +6,17 @@ Each image is one step, as in test.py:55-60: its CNOS masks stay COCO run-length
 (`preprocess.crop_detections_rle`, gp_crop_resize_pad_rle), then `GigaPose.eval_retrieval` writes the step's
 predictions/{idx}.npz, and `save_predictions_from_batched_predictions` writes the csv at the end.  A background thread
 decodes the next image into pinned memory while the current one runs.  INTEGRATION.md lists every deviation from
-test.py.  Usage:
+test.py.
+
+Row f10, `--refine-depth H`: the reference's second stage (refine.py -> pose_estimator.run_inference_pipeline,
+src/megapose/inference/pose_estimator.py:580-623) on the depth images of the split.  The first H hypotheses of every
+instance that reaches the coarse csv are refined with the point-to-plane ICP (`GigaPose.refine_depth`, no masks, as
+run_depth_refiner passes none, pose_estimator.py:501-503), the refined hypotheses are scored against the depth image
+(gp_depth_score) and the best one per instance goes to refined_predictions/{idx}.npz and a second csv,
+`..._{run_id}_icp.csv`.  The depth PNG is decoded on the thread that decodes the next RGB image.  Usage:
 
     python -m gigapose_b200.bop_run --dataset-dir D --checkpoint gigaPose_v1.ckpt --template-poses P.npy
-        [--setting localization|detection] [--detections FILE] [--out DIR] [--evaluate]
+        [--setting localization|detection] [--detections FILE] [--out DIR] [--refine-depth H] [--evaluate]
 """
 from __future__ import annotations
 
@@ -25,10 +32,11 @@ import types
 import numpy as np
 import torch
 
-from .bop_eval import load_cameras
+from .bop_eval import load_cameras, load_depth
 
 CAP_PER_TARGET = 16             # localization: detections kept per target (dataloader/test.py:110-114)
 CAP_PER_TARGET_ICBIN = 32
+TOP_K = 5                       # hypotheses per detection (configs/model/large.yaml)
 LMO_INDEX_TO_ID = [1, 5, 6, 8, 9, 10, 11, 12]      # src/utils/dataset.py: the LM-O labels the model is indexed with
 LMO_ID_TO_INDEX = {o: i + 1 for i, o in enumerate(LMO_INDEX_TO_ID)}
 
@@ -258,7 +266,7 @@ def load_checkpoint(model, path):
 
 
 def build_model(device, log_dir, checkpoint=None, seed=None):
-    """The `GigaPose` of configs/model/large.yaml (DINOv2 ViT-L/14 descriptors, ResNet IST trunk, k = 5), built in code
+    """The `GigaPose` of configs/model/large.yaml (DINOv2 ViT-L/14 descriptors, ResNet IST trunk, k = TOP_K), built in code
     as bench.build_models builds it.  With `checkpoint`, its state_dict is loaded strictly (a missing or unexpected
     key is named); `seed` seeds the initial weights (tests), otherwise they are the constructors' defaults."""
     from gigapose_b200.vit import DinoVisionTransformer
@@ -276,7 +284,7 @@ def build_model(device, log_dir, checkpoint=None, seed=None):
                            descriptor_size=256))
     reg = Regressor(descriptor_size=256, hidden_dim=256, use_tanh_act=True, normalize_output=True)
     ist = ISTNet("resnet", backbone, reg, max_batch_size=64)
-    metric = LocalSimilarity(k=5, sim_threshold=0.5, patch_threshold=3)
+    metric = LocalSimilarity(k=TOP_K, sim_threshold=0.5, patch_threshold=3)
     model = GigaPose("large", ae, ist, training_loss=None, testing_metric=metric, optim_config=None, log_interval=1000,
                      log_dir=log_dir, max_num_dets_per_forward=None)
     if checkpoint is not None:
@@ -298,23 +306,35 @@ def object_ids(dataset_dir, dataset_name):
     return ids
 
 
-def onboard(model, dataset_dir, template_poses, dataset_name=None):
-    """`GigaPose.onboard_meshes` on the dataset's meshes (models/ or models_cad/, object_ids order) with the [T,4,4]
-    template poses of INTEGRATION.md (an .npy path or an array)."""
+def read_meshes(dataset_dir, dataset_name):
+    """The dataset's meshes (models/ or models_cad/) as `read_ply` dicts, in object_ids order."""
     from gigapose_b200.render import read_ply
+    _, mname = split_name(dataset_name)
+    return [read_ply(os.path.join(dataset_dir, mname, f"obj_{o:06d}.ply"))
+            for o in object_ids(dataset_dir, dataset_name)]
+
+
+def onboard(model, dataset_dir, template_poses, dataset_name=None, meshes=None):
+    """`GigaPose.onboard_meshes` on the dataset's meshes (`read_meshes`, unless the caller already holds them) with the
+    [T,4,4] template poses of INTEGRATION.md (an .npy path or an array)."""
     name = dataset_name or os.path.basename(os.path.normpath(dataset_dir))
-    _, mname = split_name(name)
     poses = np.load(template_poses) if isinstance(template_poses, (str, os.PathLike)) else np.asarray(template_poses)
     if poses.ndim != 3 or poses.shape[1:] != (4, 4):
         raise BopRunError(f"template poses must be [T,4,4], got {poses.shape}")
-    meshes = [read_ply(os.path.join(dataset_dir, mname, f"obj_{o:06d}.ply")) for o in object_ids(dataset_dir, name)]
+    meshes = read_meshes(dataset_dir, name) if meshes is None else meshes
     return model.onboard_meshes(name, meshes, torch.as_tensor(poses, dtype=torch.float32))
 
 
 # ---------------------------------------------------------------------------------------------------- the loop
-def plan(dataset_dir, setting="localization", detections=None, dataset_name=None):
+def depth_path(dataset_dir, split, scene_id, im_id):
+    """The depth PNG `bop_eval.load_depth` reads."""
+    return os.path.join(dataset_dir, split, f"{scene_id:06d}", "depth", f"{im_id:06d}.png")
+
+
+def plan(dataset_dir, setting="localization", detections=None, dataset_name=None, depth=False):
     """Everything the loop needs from the host: dict(name, split, images [(scene, im)] in sorted order, test_list,
-    detections, cameras {scene: {im: K}})."""
+    detections, cameras {scene: {im: K}}, depth_scale {scene: {im: float}}).  With `depth`, every image's depth PNG must
+    exist: a missing one is named here, before any GPU work."""
     name = dataset_name or os.path.basename(os.path.normpath(dataset_dir))
     split, _ = split_name(name)
     path = detections or default_detections(dataset_dir)
@@ -330,36 +350,46 @@ def plan(dataset_dir, setting="localization", detections=None, dataset_name=None
             targets = json.load(f)
     test_list, selected = select_detections(dets, name, setting, targets)
     images = sorted({tuple(int(v) for v in k.split("_")) for k in test_list})
-    cams = {}
+    cams, scales = {}, {}
     for s in sorted({s for s, _ in images}):
-        cams[s] = load_cameras(dataset_dir, split, s)["K"]
+        cam = load_cameras(dataset_dir, split, s)
+        cams[s], scales[s] = cam["K"], cam["depth_scale"]
     for s, im in images:
         if im not in cams[s]:
             raise BopRunError(f"image {_key(s, im)} is not in scene_camera.json")
+        if depth and not os.path.exists(depth_path(dataset_dir, split, s, im)):
+            raise BopRunError(f"{depth_path(dataset_dir, split, s, im)} not found: depth refinement needs the depth "
+                              f"image of every test image")
     return dict(name=name, split=split, images=images, test_list=test_list, detections=selected, cameras=cams,
-                dataset_dir=dataset_dir)
+                depth_scale=scales, dataset_dir=dataset_dir)
 
 
 class _Prefetch:
-    """Decodes image i + 1 on a background thread into one of two pinned buffers while image i runs."""
+    """Decodes image i + 1 on a background thread into one of two pinned buffers while image i runs; with `depths`
+    ((dataset_dir, split, scene, im, depth_scale) per image, the arguments of `bop_eval.load_depth`), its depth image
+    too, as f32 in the model unit.  `get(i)` -> (rgb, depth or None)."""
 
-    def __init__(self, paths):
-        self.paths, self.pool, self.bufs = paths, concurrent.futures.ThreadPoolExecutor(1), {}
+    def __init__(self, paths, depths=None):
+        self.paths, self.depths = paths, depths
+        self.pool, self.bufs = concurrent.futures.ThreadPoolExecutor(1), {}
         self.next = self.pool.submit(self._load, 0) if paths else None
 
-    def _load(self, i):
-        a = read_image(self.paths[i])
-        key = (i % 2, a.shape)
+    def _pinned(self, i, a, dtype):
+        key = (i % 2, a.shape, dtype)
         buf = self.bufs.get(key)
         if buf is None:
-            buf = self.bufs[key] = torch.empty(a.shape, dtype=torch.uint8, pin_memory=True)
+            buf = self.bufs[key] = torch.empty(a.shape, dtype=dtype, pin_memory=True)
         buf.numpy()[...] = a
         return buf
 
+    def _load(self, i):
+        rgb = self._pinned(i, read_image(self.paths[i]), torch.uint8)
+        return rgb, None if self.depths is None else self._pinned(i, load_depth(*self.depths[i]), torch.float32)
+
     def get(self, i):
-        buf = self.next.result()
+        bufs = self.next.result()
         self.next = self.pool.submit(self._load, i + 1) if i + 1 < len(self.paths) else None
-        return buf
+        return bufs
 
     def close(self):
         self.pool.shutdown(wait=True)
@@ -389,36 +419,107 @@ def image_batch(p, i, rgb, device):
 
 
 @torch.no_grad()
+def refine_image(model, p, i, kept, depth, hypotheses, out_dir):
+    """Row f10 for image i of the plan: the first `hypotheses` poses of each of the `kept` instances (the collection
+    `eval_retrieval` returns after its filter, with `time` and `detection_time`) go through
+    `GigaPose.refine_depth(rank=True)` against `depth` (f32 [H,W] in the model unit, host or device), and
+    out_dir/refined_predictions/{i}.npz takes, per instance, the pose of its best hypothesis, that hypothesis' coarse
+    score, the dataset's object id, `time` = the image's coarse time (detection + retrieval) and `refinement_time`,
+    measured with CUDA events from the depth upload to the end of the scoring, plus `hypothesis` (the index chosen) and
+    its `icp_status`, which the csv writer does not read.  -> the refined collection."""
+    s, im = p["images"][i]
+    device = kept.pred_poses.device
+    n = len(kept)
+    start, stop = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    start.record()
+    depth = torch.as_tensor(depth).to(device, non_blocking=True)
+    K = torch.as_tensor(p["cameras"][s][im], dtype=torch.float64).float()
+    refined = model.refine_depth(p["name"], kept, depth[None], frame_idx=np.zeros(n, np.int64), hypotheses=hypotheses,
+                                 K=K, rank=True)
+    rows = torch.arange(n, device=device)
+    poses = refined.pred_poses[rows, refined.best_hypothesis]
+    scores = kept.scores[rows, refined.best_hypothesis]
+    status = refined.icp_status[rows, refined.best_hypothesis]
+    stop.record()
+    stop.synchronize()
+    labels = np.asarray(kept.infos.label).astype(np.int32)
+    if "lmo" in p["name"]:
+        labels = np.asarray(LMO_INDEX_TO_ID, np.int32)[labels - 1]
+    coarse_time = (kept.time + kept.detection_time).cpu().numpy()
+    os.makedirs(os.path.join(out_dir, "refined_predictions"), exist_ok=True)
+    np.savez(os.path.join(out_dir, "refined_predictions", f"{i}.npz"),
+             scene_id=np.asarray(kept.infos.scene_id).astype(np.int32),
+             im_id=np.asarray(kept.infos.view_id).astype(np.int32), object_id=labels, time=coarse_time,
+             refinement_time=np.full(n, start.elapsed_time(stop) / 1e3), poses=poses.cpu().numpy(),
+             scores=scores.cpu().numpy(), hypothesis=refined.best_hypothesis.cpu().numpy(),
+             icp_status=status.cpu().numpy())
+    return refined
+
+
+@torch.no_grad()
 def run(model, dataset_dir, out_dir, setting="localization", detections=None, template_poses=None, run_id="bop_run",
-        dataset_name=None):
+        dataset_name=None, refine_hypotheses=0):
     """Runs the test split: onboards the dataset from `template_poses` unless the model already holds it, then one
     `eval_retrieval` per image (predictions under out_dir/predictions, which must hold no .npz yet) and the csv.
-    -> path of the csv (`{model}-pbrreal-rgb-mmodel_{dataset}-test_{run_id}.csv` in out_dir/predictions)."""
+    -> path of the csv (`{model}-pbrreal-rgb-mmodel_{dataset}-test_{run_id}.csv` in out_dir/predictions).
+    With `refine_hypotheses` = H in 1 .. k, each image's kept instances also go through `refine_image` with the image's
+    depth PNG, and a second csv (`..._{run_id}_icp.csv` in out_dir/refined_predictions) is written
+    -> (coarse csv, refined csv)."""
     from src.utils.inout import save_predictions_from_batched_predictions
-    p = plan(dataset_dir, setting, detections, dataset_name)
-    pred_dir = os.path.join(out_dir, "predictions")
+    H = int(refine_hypotheses)
+    if not 0 <= H <= model.testing_metric.k:
+        raise BopRunError(f"refine_hypotheses {H} outside [0, {model.testing_metric.k}]")
+    p = plan(dataset_dir, setting, detections, dataset_name, depth=H > 0)
+    pred_dir, ref_dir = os.path.join(out_dir, "predictions"), os.path.join(out_dir, "refined_predictions")
     os.makedirs(pred_dir, exist_ok=True)
-    if glob.glob(os.path.join(glob.escape(pred_dir), "*.npz")):
-        raise BopRunError(f"{pred_dir} already holds prediction files; use an empty --out")
-    if p["name"] not in model.engines:
-        if template_poses is None:
-            raise BopRunError(f"{p['name']} is not onboarded and no template poses were given")
-        onboard(model, dataset_dir, template_poses, p["name"])
+    for d in (pred_dir, ref_dir):
+        if glob.glob(os.path.join(glob.escape(d), "*.npz")):
+            raise BopRunError(f"{d} already holds prediction files; use an empty --out")
+    name = p["name"]
+    attach = H > 0 and name not in getattr(model, "meshes", {})
+    if name not in model.engines and template_poses is None:
+        raise BopRunError(f"{name} is not onboarded and no template poses were given")
+    meshes = read_meshes(dataset_dir, name) if attach or name not in model.engines else None
+    if name not in model.engines:
+        onboard(model, dataset_dir, template_poses, name, meshes)
+    if attach:
+        model.attach_meshes(name, meshes)
     model.log_dir = out_dir
-    device = model.engines[p["name"]].device
-    pre = _Prefetch([image_path(dataset_dir, p["split"], s, im) for s, im in p["images"]])
+    device = model.engines[name].device
+    pre = _Prefetch([image_path(dataset_dir, p["split"], s, im) for s, im in p["images"]],
+                    [(dataset_dir, p["split"], s, im, p["depth_scale"][s][im]) for s, im in p["images"]] if H else None)
     try:
         for i in range(len(p["images"])):
-            batch = image_batch(p, i, pre.get(i), device)
-            model.eval_retrieval(batch, idx_batch=i, dataset_name=p["name"])
+            rgb, depth = pre.get(i)
+            batch = image_batch(p, i, rgb, device)
+            _, kept = model.eval_retrieval(batch, idx_batch=i, dataset_name=name)
+            if H:
+                refine_image(model, p, i, kept, depth, H, out_dir)
     finally:
         pre.close()
-    save_predictions_from_batched_predictions(pred_dir, dataset_name=p["name"], model_name=model.model_name,
+    stem = f"{model.model_name}-pbrreal-rgb-mmodel_{name}-test_{run_id}"
+    save_predictions_from_batched_predictions(pred_dir, dataset_name=name, model_name=model.model_name,
                                               run_id=run_id, is_refined=False)
-    return os.path.join(pred_dir, f"{model.model_name}-pbrreal-rgb-mmodel_{p['name']}-test_{run_id}.csv")
+    coarse = os.path.join(pred_dir, f"{stem}.csv")
+    if not H:
+        return coarse
+    save_predictions_from_batched_predictions(ref_dir, dataset_name=name, model_name=model.model_name,
+                                              run_id=f"{run_id}_icp", is_refined=True)
+    return coarse, os.path.join(ref_dir, f"{stem}_icp.csv")
 
 
-def main(argv=None):
+def _evaluate(csv, dataset_dir, setting, out_dir, device):
+    from . import bop_eval
+    split, _ = split_name(os.path.basename(os.path.normpath(dataset_dir)))
+    if setting == "localization":
+        res = bop_eval.evaluate(csv, dataset_dir, split, out_dir=out_dir, device=device)
+        print(json.dumps({k: res[k] for k in ("ar", "ar_vsd", "ar_mssd", "ar_mspd", "n_targets")}))
+    else:
+        res = bop_eval.evaluate_detection(csv, dataset_dir, split, out_dir=out_dir, device=device)
+        print(json.dumps({k: res[k] for k in ("map", "map_mssd", "map_mspd")}))
+
+
+def parser():
     ap = argparse.ArgumentParser(description="GigaPose on a BOP test split with its CNOS detections -> BOP results csv")
     ap.add_argument("--dataset-dir", required=True, help="BOP dataset directory, e.g. <root>/lmo")
     ap.add_argument("--checkpoint", required=True, help="Lightning checkpoint (gigaPose_v1.ckpt)")
@@ -426,21 +527,23 @@ def main(argv=None):
     ap.add_argument("--setting", choices=("localization", "detection"), default="localization")
     ap.add_argument("--detections", default=None, help="CNOS detections json (default: <root>/default_detections/...)")
     ap.add_argument("--out", default="bop_run_out")
-    ap.add_argument("--evaluate", action="store_true", help="score the csv with bop_eval")
+    ap.add_argument("--refine-depth", type=int, default=0, choices=range(TOP_K + 1), metavar="H",
+                    help=f"refine the first H (1..{TOP_K}) hypotheses of every kept instance against the depth images "
+                         f"and write a second csv with the best one (0: no refinement)")
+    ap.add_argument("--evaluate", action="store_true", help="score the csv (both, coarse first, when refining) with bop_eval")
     ap.add_argument("--device", default="cuda")
-    a = ap.parse_args(argv)
+    return ap
+
+
+def main(argv=None):
+    a = parser().parse_args(argv)
     model = build_model(a.device, a.out, checkpoint=a.checkpoint)
-    csv = run(model, a.dataset_dir, a.out, a.setting, a.detections, a.template_poses)
-    print(csv)
-    if a.evaluate:
-        from . import bop_eval
-        split, _ = split_name(os.path.basename(os.path.normpath(a.dataset_dir)))
-        if a.setting == "localization":
-            res = bop_eval.evaluate(csv, a.dataset_dir, split, out_dir=a.out, device=a.device)
-            print(json.dumps({k: res[k] for k in ("ar", "ar_vsd", "ar_mssd", "ar_mspd", "n_targets")}))
-        else:
-            res = bop_eval.evaluate_detection(csv, a.dataset_dir, split, out_dir=a.out, device=a.device)
-            print(json.dumps({k: res[k] for k in ("map", "map_mssd", "map_mspd")}))
+    csvs = run(model, a.dataset_dir, a.out, a.setting, a.detections, a.template_poses, refine_hypotheses=a.refine_depth)
+    csvs = (csvs,) if isinstance(csvs, str) else csvs
+    for csv, out in zip(csvs, (a.out, os.path.join(a.out, "refined"))):
+        print(csv)
+        if a.evaluate:
+            _evaluate(csv, a.dataset_dir, a.setting, out, a.device)
 
 
 if __name__ == "__main__":

@@ -2,7 +2,9 @@
 (`gp_render_templates`), the measured depth of each frame becomes an organised target map with normals
 (`gp_icp_prepare_scene`), and one CTA per hypothesis runs the centroid shift and a point-to-plane ICP
 (`gp_icp_refine`).  csrc/depth_icp.cu's header comment states the contract; it restates MegaPose's ICPRefiner
-(src/megapose/inference/icp_refiner.py:134-287) with the deviations listed in INTEGRATION.md."""
+(src/megapose/inference/icp_refiner.py:134-287) with the deviations listed in INTEGRATION.md.  Row f10:
+`score_hypotheses` renders final poses the same way and scores them against the measured depth (`gp_depth_score`,
+csrc/depth_score.cu), so that the best hypothesis of a detection can be kept."""
 from __future__ import annotations
 
 import ctypes as C
@@ -94,21 +96,12 @@ def refine_rendered(depth, K, frame_idx, rendered, boxes, poses, masks, workspac
     return out, status, residual, fitness
 
 
-@torch.no_grad()
-def refine_icp(meshes_dev, labels, poses, depth, K, frame_idx, masks=None, **params):
-    """Refines n hypotheses against the measured depth.
-
-    meshes_dev  list of device meshes (`device_meshes`), indexed by labels [n] (0-based);
-    poses       [n,4,4] coarse object -> camera poses, in the depth unit;
-    depth       [F,H,W] measured depth (0 = missing), K [F,3,3] full-image intrinsics, frame_idx [n] frame of each;
-    masks       None (the reference's threshold rule) or [n,H,W] full-frame detection masks;
-    params      see DEFAULTS (unit_per_m = 1000 for mm).
-    -> (poses [n,4,4], status [n] i32 (STATUS_NAMES), residual [n], fitness [n]) on the device; a pose whose status is
-    not 0 is its input pose bit for bit."""
+def _inputs(what, meshes_dev, labels, poses, depth, K, frame_idx):
+    """The checked inputs `refine_icp` and `score_hypotheses` share: poses f32 [n,4,4], depth f32 [F,H,W] and K f32
+    [F,3,3] on the poses' device, labels and frame_idx i64 [n] on the host."""
     device = poses.device
     if device.type != "cuda":
-        raise _lib.GigaPoseNativeError("refine_icp runs on CUDA devices only (no CPU fallback)")
-    upm = float(params.get("unit_per_m", DEFAULTS["unit_per_m"]))
+        raise _lib.GigaPoseNativeError(f"{what} runs on CUDA devices only (no CPU fallback)")
     poses = poses.to(device, torch.float32).reshape(-1, 4, 4).contiguous()
     depth = torch.as_tensor(depth).to(device, torch.float32).contiguous()
     if depth.dim() == 2:
@@ -127,6 +120,25 @@ def refine_icp(meshes_dev, labels, poses, depth, K, frame_idx, masks=None, **par
         raise ValueError(f"labels outside [0, {len(meshes_dev)})")
     if n and (int(frame_idx.min()) < 0 or int(frame_idx.max()) >= F):
         raise ValueError(f"frame_idx outside [0, {F})")
+    return poses, depth, K, labels, frame_idx
+
+
+@torch.no_grad()
+def refine_icp(meshes_dev, labels, poses, depth, K, frame_idx, masks=None, **params):
+    """Refines n hypotheses against the measured depth.
+
+    meshes_dev  list of device meshes (`device_meshes`), indexed by labels [n] (0-based);
+    poses       [n,4,4] coarse object -> camera poses, in the depth unit;
+    depth       [F,H,W] measured depth (0 = missing), K [F,3,3] full-image intrinsics, frame_idx [n] frame of each;
+    masks       None (the reference's threshold rule) or [n,H,W] full-frame detection masks;
+    params      see DEFAULTS (unit_per_m = 1000 for mm).
+    -> (poses [n,4,4], status [n] i32 (STATUS_NAMES), residual [n], fitness [n]) on the device; a pose whose status is
+    not 0 is its input pose bit for bit."""
+    upm = float(params.get("unit_per_m", DEFAULTS["unit_per_m"]))
+    poses, depth, K, labels, frame_idx = _inputs("refine_icp", meshes_dev, labels, poses, depth, K, frame_idx)
+    device = poses.device
+    F, H, W = depth.shape
+    n = poses.shape[0]
     if masks is not None:
         masks = torch.as_tensor(masks).to(device).reshape(n, H, W).to(torch.uint8).contiguous()
     out = poses.clone()
@@ -148,3 +160,40 @@ def refine_icp(meshes_dev, labels, poses, depth, K, frame_idx, masks=None, **par
                             None if masks is None else masks[sl], ws, **params)
         out[sl], status[sl], residual[sl], fitness[sl] = o
     return out, status, residual, fitness
+
+
+@torch.no_grad()
+def score_hypotheses(meshes_dev, labels, poses, depth, K, frame_idx, n_hyp, tolerance_m=0.015, unit_per_m=1000.0):
+    """Depth-consistency score of n = n_det * n_hyp poses (row d * n_hyp + j is hypothesis j of detection d; labels,
+    poses, depth, K and frame_idx as `refine_icp` takes them, the hypotheses of a detection sharing one frame): every
+    pose is rendered with `render_hypotheses`, the renderer call the ICP's sources come from, and gp_depth_score counts
+    the rendered pixels whose measured depth is within `tolerance_m` (VSD's visibility tolerance, 15 mm), behind it, in
+    front of it or missing (csrc/depth_score.cu's header comment states the contract).
+    -> (counts [n,4] i32 = consistent, behind, front, missing; score [n] = consistent / (consistent + behind + front);
+    best [n_det] i32, the hypothesis with the largest score, the lowest index on a tie) on the device."""
+    n_hyp = int(n_hyp)
+    if n_hyp < 1:
+        raise ValueError(f"n_hyp {n_hyp} must be >= 1")
+    poses, depth, K, labels, frame_idx = _inputs("score_hypotheses", meshes_dev, labels, poses, depth, K, frame_idx)
+    device = poses.device
+    F, H, W = depth.shape
+    n = poses.shape[0]
+    if n % n_hyp:
+        raise ValueError(f"{n} poses are not a whole number of groups of {n_hyp} hypotheses")
+    n_det = n // n_hyp
+    if not torch.equal(frame_idx, frame_idx[::n_hyp].repeat_interleave(n_hyp)):
+        raise ValueError("the hypotheses of a detection must share one frame")
+    counts = torch.empty(n, 4, dtype=torch.int32, device=device)
+    score = torch.empty(n, device=device)
+    best = torch.empty(n_det, dtype=torch.int32, device=device)
+    fi = frame_idx[::n_hyp].to(device, torch.int32)
+    chunk = max(1, min(n_det, WORKSPACE_BYTES // (52 * H * W * n_hyp)))      # detections per chunk, renders as above
+    for s in range(0, n_det, chunk):
+        e = min(n_det, s + chunk)
+        sl = slice(s * n_hyp, e * n_hyp)
+        rendered, boxes = render_hypotheses(meshes_dev, labels[sl], poses[sl], K, frame_idx[sl], H, W, unit_per_m)
+        check(_lib.load().gp_depth_score(F, e - s, n_hyp, H, W, fi[s:e].data_ptr(), depth.data_ptr(),
+                                         rendered.data_ptr(), boxes.data_ptr(), float(tolerance_m) * float(unit_per_m),
+                                         counts[sl].data_ptr(), score[sl].data_ptr(), best[s:e].data_ptr(),
+                                         torch.cuda.current_stream(device).cuda_stream))
+    return counts, score, best

@@ -450,6 +450,18 @@ int gp_icp_refine(int n_frames, int n_hyp, int height, int width, const int32_t*
  * 0 <= rank < n; arguments are checked before any device work. */
 int gp_debug_icp_select(const uint32_t* bits, int n, int rank, uint32_t* out, void* stream);
 
+/* --- row f10: depth-consistency score of the hypotheses of each detection, and the best one.  The full contract is the
+ * header comment of gigapose_b200/csrc/depth_score.cu.  Needs no handle. ------------------------------------------ */
+/* frame_idx i32 [n_det]; depth f32 [n_frames,H,W] measured (not > 0 = missing); rendered f32 [n_det*n_hyp,H,W] the
+ * render of each pose (0 = background) and boxes i64 [n_det*n_hyp,4] as gp_render_templates writes them, hypothesis j
+ * of detection d at row d * n_hyp + j; tolerance >= 0 in the depth unit.  Outputs: counts i32 [n_det*n_hyp,4] =
+ * (consistent, behind, front, missing) over the rendered pixels, score f32 [n_det*n_hyp] = consistent / (consistent +
+ * behind + front) (0 for an empty denominator), best i32 [n_det] = the hypothesis with the largest score, the lowest
+ * index on a tie.  A detection whose frame index is out of range gets counts -1, scores NaN and best -1. */
+int gp_depth_score(int n_frames, int n_det, int n_hyp, int height, int width, const int32_t* frame_idx,
+                   const float* depth, const float* rendered, const int64_t* boxes, float tolerance, int32_t* counts,
+                   float* score, int32_t* best, void* stream);
+
 /* --- diagnostics ----------------------------------------------------------------------------------------- */
 /* number of kernels this library has launched since load (all handles); used for bench.py's `gpu_launches` */
 uint64_t gp_launch_count(void);

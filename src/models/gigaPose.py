@@ -280,7 +280,7 @@ class GigaPose(LightningModule):
 
     @torch.no_grad()
     def refine_depth(self, dataset_name, predictions, depth, frame_idx=None, masks=None, hypotheses=1, *, K=None,
-                     **params):
+                     rank=False, **params):
         """MegaPose's ICPRefiner.refine_poses on the output of `retrieve()`: the first `hypotheses` of the k poses of every
         detection are rendered and refined against the measured depth (gigapose_b200.icp.refine_icp).
 
@@ -291,8 +291,12 @@ class GigaPose(LightningModule):
         indexed by detection, not by frame (pass `tar_K[i]` of one detection i per frame); params as
         gigapose_b200.icp.DEFAULTS.  Returns a new collection: `pred_poses` replaced where the
         refinement was accepted (same order, nothing re-sorted), `poses_input` the coarse poses, and `icp_status`,
-        `icp_residual`, `icp_fitness` [B,hypotheses]."""
-        from gigapose_b200.icp import refine_icp
+        `icp_residual`, `icp_fitness` [B,hypotheses].  With `rank=True` the final poses (refined where accepted, coarse
+        where not) are also scored against the depth (gigapose_b200.icp.score_hypotheses, row f10) and the collection
+        carries `depth_counts` [B,hypotheses,4] (consistent, behind, front, missing pixels), `depth_score`
+        [B,hypotheses] and `best_hypothesis` [B] (int64: the highest score, the lowest index on a tie); the order of the
+        hypotheses still does not change."""
+        from gigapose_b200.icp import DEFAULTS, refine_icp, score_hypotheses
         if K is None:
             raise TypeError("refine_depth needs K=, the frames' full-image intrinsics [F,3,3] or [3,3]")
         meshes = self.meshes[dataset_name]
@@ -322,6 +326,12 @@ class GigaPose(LightningModule):
         refined.register_tensor("icp_status", status.reshape(B, h))
         refined.register_tensor("icp_residual", residual.reshape(B, h))
         refined.register_tensor("icp_fitness", fitness.reshape(B, h))
+        if rank:
+            counts, score, best = score_hypotheses(meshes, np.repeat(labels, h), out, depth, K, np.repeat(frame_idx, h), h,
+                                                   unit_per_m=params.get("unit_per_m", DEFAULTS["unit_per_m"]))
+            refined.register_tensor("depth_counts", counts.reshape(B, h, 4))
+            refined.register_tensor("depth_score", score.reshape(B, h))
+            refined.register_tensor("best_hypothesis", best.to(torch.int64))
         return refined
 
     # ------------------------------------------------------------------ localisation filter + writer (gigaPose.py:400-449)
