@@ -90,6 +90,12 @@ class GpIcpParams(C.Structure):
                 ("min_step_rad", C.c_float), ("min_step_m", C.c_float), ("debug", GpIcpDebug)]
 
 
+class GpIcpMaskSet(C.Structure):
+    """gp_icp_mask_set_t: the HOST description of the detections of the masked mode."""
+    _fields_ = [("n_det", C.c_int32), ("frame", C.POINTER(C.c_int32)), ("boxes", C.POINTER(C.c_int32)),
+                ("run_offsets", C.POINTER(C.c_int64))]
+
+
 # gp_icp_refine statuses (GP_ICP_*)
 ICP_OK, ICP_TOO_FEW_POINTS, ICP_DEGENERATE, ICP_RESIDUAL, ICP_INVALID, ICP_LOST = 0, 1, 2, 3, 4, 5
 
@@ -161,6 +167,16 @@ SYMBOLS = {
     "gp_icp_refine": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                 C.c_void_p, C.c_void_p, C.POINTER(GpIcpParams), C.c_void_p, C.c_void_p, C.c_void_p,
                                 C.c_void_p, C.c_void_p, C.c_void_p]),
+    "gp_icp_masked_query_sizes": (C.c_int, [C.c_int, C.c_int, C.c_int, C.POINTER(GpIcpMaskSet), C.POINTER(C.c_size_t),
+                                            C.POINTER(C.c_int64), C.POINTER(C.c_size_t), C.POINTER(C.c_size_t)]),
+    "gp_icp_masked_decode": (C.c_int, [C.c_int, C.c_int, C.c_int, C.POINTER(GpIcpMaskSet), C.c_void_p, C.c_void_p,
+                                       C.c_void_p, C.c_void_p]),
+    "gp_icp_prepare_masked_scene": (C.c_int, [C.c_int, C.c_int, C.c_int, C.POINTER(GpIcpMaskSet), C.c_void_p,
+                                              C.c_void_p, C.c_float, C.c_void_p, C.c_void_p]),
+    "gp_icp_refine_masked": (C.c_int, [C.c_int, C.c_int, C.c_int, C.POINTER(GpIcpMaskSet), C.c_int, C.c_void_p,
+                                       C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(GpIcpParams),
+                                       C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                       C.c_void_p]),
     "gp_debug_icp_select": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
     "gp_depth_score": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
                                  C.c_void_p, C.c_float, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),

@@ -13,10 +13,15 @@ src/megapose/inference/pose_estimator.py:580-623) on the depth images of the spl
 instance that reaches the coarse csv are refined with the point-to-plane ICP (`GigaPose.refine_depth`, no masks, as
 run_depth_refiner passes none, pose_estimator.py:501-503), the refined hypotheses are scored against the depth image
 (gp_depth_score) and the best one per instance goes to refined_predictions/{idx}.npz and a second csv,
-`..._{run_id}_icp.csv`.  The depth PNG is decoded on the thread that decodes the next RGB image.  Usage:
+`..._{run_id}_icp.csv`.  The depth PNG is decoded on the thread that decodes the next RGB image.
+
+Row f11, `--refine-masks` with `--refine-depth H`: each kept instance is refined with its own CNOS mask, the run-length
+encoding decoded on the GPU over the mask's box, as the target set and as the region its target normals are smoothed
+in (`GigaPose.refine_depth(mask_normals=True)`); the csv is `..._{run_id}_icp_masked.csv`.  Usage:
 
     python -m gigapose_b200.bop_run --dataset-dir D --checkpoint gigaPose_v1.ckpt --template-poses P.npy
-        [--setting localization|detection] [--detections FILE] [--out DIR] [--refine-depth H] [--evaluate]
+        [--setting localization|detection] [--detections FILE] [--out DIR] [--refine-depth H [--refine-masks]]
+        [--evaluate]
 """
 from __future__ import annotations
 
@@ -415,18 +420,29 @@ def image_batch(p, i, rgb, device):
     batch.test_list = tc.PandasTensorCollection(infos=pd.DataFrame(dict(
         im_id=[im] * len(x["obj_id"]), scene_id=[s] * len(x["obj_id"]), obj_id=x["obj_id"],
         inst_count=x["inst_count"], detection_time=[x["detection_time"]] * len(x["obj_id"]))))
+    batch.rle = (x["counts"], x["offsets"])
     return batch
 
 
+def select_rle(rle, selected):
+    """The (counts, offsets) of the detections `selected` (indices into the image's detections), in that order."""
+    counts, off = rle
+    parts = [counts[off[i]:off[i + 1]] for i in selected]
+    return (np.concatenate(parts) if parts else np.zeros(0, np.int32),
+            np.concatenate([[0], np.cumsum([len(c) for c in parts])]).astype(np.int64))
+
+
 @torch.no_grad()
-def refine_image(model, p, i, kept, depth, hypotheses, out_dir):
+def refine_image(model, p, i, kept, depth, hypotheses, out_dir, masks=None):
     """Row f10 for image i of the plan: the first `hypotheses` poses of each of the `kept` instances (the collection
     `eval_retrieval` returns after its filter, with `time` and `detection_time`) go through
     `GigaPose.refine_depth(rank=True)` against `depth` (f32 [H,W] in the model unit, host or device), and
     out_dir/refined_predictions/{i}.npz takes, per instance, the pose of its best hypothesis, that hypothesis' coarse
     score, the dataset's object id, `time` = the image's coarse time (detection + retrieval) and `refinement_time`,
     measured with CUDA events from the depth upload to the end of the scoring, plus `hypothesis` (the index chosen) and
-    its `icp_status`, which the csv writer does not read.  -> the refined collection."""
+    its `icp_status`, which the csv writer does not read.  With `masks` = (counts, offsets), the run-length masks of
+    the kept instances in their order, they refine with `mask_normals=True`; `refinement_time` then covers the mask
+    decode.  -> the refined collection."""
     s, im = p["images"][i]
     device = kept.pred_poses.device
     n = len(kept)
@@ -434,8 +450,9 @@ def refine_image(model, p, i, kept, depth, hypotheses, out_dir):
     start.record()
     depth = torch.as_tensor(depth).to(device, non_blocking=True)
     K = torch.as_tensor(p["cameras"][s][im], dtype=torch.float64).float()
+    extra = {} if masks is None else dict(masks=dict(counts=masks[0], offsets=masks[1]), mask_normals=True)
     refined = model.refine_depth(p["name"], kept, depth[None], frame_idx=np.zeros(n, np.int64), hypotheses=hypotheses,
-                                 K=K, rank=True)
+                                 K=K, rank=True, **extra)
     rows = torch.arange(n, device=device)
     poses = refined.pred_poses[rows, refined.best_hypothesis]
     scores = kept.scores[rows, refined.best_hypothesis]
@@ -458,17 +475,20 @@ def refine_image(model, p, i, kept, depth, hypotheses, out_dir):
 
 @torch.no_grad()
 def run(model, dataset_dir, out_dir, setting="localization", detections=None, template_poses=None, run_id="bop_run",
-        dataset_name=None, refine_hypotheses=0):
+        dataset_name=None, refine_hypotheses=0, refine_masks=False):
     """Runs the test split: onboards the dataset from `template_poses` unless the model already holds it, then one
     `eval_retrieval` per image (predictions under out_dir/predictions, which must hold no .npz yet) and the csv.
     -> path of the csv (`{model}-pbrreal-rgb-mmodel_{dataset}-test_{run_id}.csv` in out_dir/predictions).
     With `refine_hypotheses` = H in 1 .. k, each image's kept instances also go through `refine_image` with the image's
     depth PNG, and a second csv (`..._{run_id}_icp.csv` in out_dir/refined_predictions) is written
-    -> (coarse csv, refined csv)."""
+    -> (coarse csv, refined csv).  With `refine_masks` they refine with their own CNOS masks (`refine_image`'s masks)
+    and the second csv is `..._{run_id}_icp_masked.csv`."""
     from src.utils.inout import save_predictions_from_batched_predictions
     H = int(refine_hypotheses)
     if not 0 <= H <= model.testing_metric.k:
         raise BopRunError(f"refine_hypotheses {H} outside [0, {model.testing_metric.k}]")
+    if refine_masks and not H:
+        raise BopRunError("refine_masks needs refine_hypotheses >= 1")
     p = plan(dataset_dir, setting, detections, dataset_name, depth=H > 0)
     pred_dir, ref_dir = os.path.join(out_dir, "predictions"), os.path.join(out_dir, "refined_predictions")
     os.makedirs(pred_dir, exist_ok=True)
@@ -492,9 +512,10 @@ def run(model, dataset_dir, out_dir, setting="localization", detections=None, te
         for i in range(len(p["images"])):
             rgb, depth = pre.get(i)
             batch = image_batch(p, i, rgb, device)
-            _, kept = model.eval_retrieval(batch, idx_batch=i, dataset_name=name)
+            selected, kept = model.eval_retrieval(batch, idx_batch=i, dataset_name=name)
             if H:
-                refine_image(model, p, i, kept, depth, H, out_dir)
+                refine_image(model, p, i, kept, depth, H, out_dir,
+                             select_rle(batch.rle, selected) if refine_masks else None)
     finally:
         pre.close()
     stem = f"{model.model_name}-pbrreal-rgb-mmodel_{name}-test_{run_id}"
@@ -503,9 +524,10 @@ def run(model, dataset_dir, out_dir, setting="localization", detections=None, te
     coarse = os.path.join(pred_dir, f"{stem}.csv")
     if not H:
         return coarse
+    suffix = "_icp_masked" if refine_masks else "_icp"
     save_predictions_from_batched_predictions(ref_dir, dataset_name=name, model_name=model.model_name,
-                                              run_id=f"{run_id}_icp", is_refined=True)
-    return coarse, os.path.join(ref_dir, f"{stem}_icp.csv")
+                                              run_id=f"{run_id}{suffix}", is_refined=True)
+    return coarse, os.path.join(ref_dir, f"{stem}{suffix}.csv")
 
 
 def _evaluate(csv, dataset_dir, setting, out_dir, device):
@@ -530,6 +552,9 @@ def parser():
     ap.add_argument("--refine-depth", type=int, default=0, choices=range(TOP_K + 1), metavar="H",
                     help=f"refine the first H (1..{TOP_K}) hypotheses of every kept instance against the depth images "
                          f"and write a second csv with the best one (0: no refinement)")
+    ap.add_argument("--refine-masks", action="store_true",
+                    help="with --refine-depth: refine each instance with its own CNOS mask, target normals smoothed "
+                         "within it (writes ..._icp_masked.csv)")
     ap.add_argument("--evaluate", action="store_true", help="score the csv (both, coarse first, when refining) with bop_eval")
     ap.add_argument("--device", default="cuda")
     return ap
@@ -537,8 +562,11 @@ def parser():
 
 def main(argv=None):
     a = parser().parse_args(argv)
+    if a.refine_masks and not a.refine_depth:
+        parser().error("--refine-masks needs --refine-depth H")
     model = build_model(a.device, a.out, checkpoint=a.checkpoint)
-    csvs = run(model, a.dataset_dir, a.out, a.setting, a.detections, a.template_poses, refine_hypotheses=a.refine_depth)
+    csvs = run(model, a.dataset_dir, a.out, a.setting, a.detections, a.template_poses, refine_hypotheses=a.refine_depth,
+               refine_masks=a.refine_masks)
     csvs = (csvs,) if isinstance(csvs, str) else csvs
     for csv, out in zip(csvs, (a.out, os.path.join(a.out, "refined"))):
         print(csv)

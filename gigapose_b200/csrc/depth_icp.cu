@@ -43,12 +43,34 @@
 // Layout: three scene kernels (vertical pass, horizontal pass, normals) over all frames; one persistent CTA per
 // hypothesis runs stages 2-6 without host synchronisation.  A hypothesis' result depends on its own inputs only.
 //
+// Masked normals (row f11, opt-in; the reference smooths the whole frame).  Detection d has a frame f, the measured
+// depth D of f and a mask M_d, given dense or as COCO run-length encoding.
+//  1'. Smoothing within the mask: S_d = (G * (D [D > 0] M_d)) / (G * ([D > 0] M_d)), the same G, vertical pass first,
+//      scipy's `reflect` at the frame border, and the fp32 operation order of smooth_v_kernel / smooth_u_kernel.
+//      Gradients and normals are stage 1's, taken from S_d; points are back-projected from the raw D as in stage 1.
+//  2'. Target set: map z > 0 and M_d (stage 2's mask rule), counted over the mask's box.
+//  Stages 3-6 are unchanged; hypothesis i reads the map and mask of detection det_idx[i], so the hypotheses of a
+//  detection share them.
+//  Consequences: with M_d = 1 over the frame the map is stage 1's bit for bit (skipping a weight-0 pixel adds +0).
+//  Outside M_d every weight is 0, so S_d anywhere depends only on D inside the mask's bounding box [x0, x1) x [y0, y1),
+//  and the map at the box's pixels only on S_d within 2 px of the box (the gradient stencil, one-sided at the frame
+//  border).  So S_d is computed on the box grown by kMargin = 2 px and clipped to the frame ("ext"), the map and the
+//  mask on the box itself, with box-relative addressing: memory scales with the box areas, not with H * W per
+//  detection.  Layout: gp_icp_masked_decode writes the detection table and decodes each mask into a u8 box tile
+//  (run-length masks: rle_scan_kernel's running sums, then the parity of the upper bound at col * H + row);
+//  gp_icp_prepare_masked_scene runs three kernels over the ext tiles and boxes of all detections;
+//  gp_icp_refine_masked is icp_kernel<true>, whose targets are looked up in the box tiles and whose scratch is
+//  box-sized.  A pixel outside the box reads as 0 even where a dense mask is set: the box must contain the mask.
+//
 // Debug hooks (tests/test_gpu_icp_solver.py): with debug.trace set, thread 0 writes one gp_icp_trace_t per iteration
 // (the fp32 transform it associated with, the counts, the median, the 29 fp64 sums, the step and the correction after
 // it), so that each step can be checked against an fp64 reference started from the kernel's own state; the outputs are
 // the same with and without it.  gp_debug_icp_select runs the median's radix_select alone.
 #include "../../include/gigapose_b200.h"
 #include "gigapose_kernels.h"
+
+#include <algorithm>
+#include <vector>
 
 using gp::fail;
 
@@ -63,6 +85,17 @@ constexpr int kMaxLevels = 8;
 constexpr int kMinSide = 2 * kRadius + 1;
 constexpr int kMaxSide = 8192;
 constexpr unsigned kNoPair = 0x7f800000u;  // +inf bits: sorts after every distance
+constexpr int kMargin = 2;               // ext = mask box + kMargin px: the gradient stencil, one-sided at the border
+
+struct MaskDet {          // one detection of the masked mode (device table at the start of the masked workspace)
+  int box[4];             // mask box x0, y0, x1, y1 (exclusive max); empty when x1 <= x0 or y1 <= y0
+  int ext[4];             // the box grown by kMargin and clipped to the frame (empty with the box)
+  int frame;
+  int reserved;
+  long long tile;         // first entry of its mask tile (u8) and map (f32 x 6), box-relative row-major
+  long long ext_off;      // first entry of its num / den / S tiles, ext-relative row-major
+  long long run0, run1;   // its runs in counts / ends (run-length masks)
+};
 
 __device__ __forceinline__ int reflect(int i, int n) {   // scipy 'reflect' (d c b a | a b c d | d c b a), n > kRadius
   return i < 0 ? -i - 1 : i >= n ? 2 * n - i - 1 : i;
@@ -117,27 +150,20 @@ smooth_u_kernel(int H, int W, const float* __restrict__ num, const float* __rest
 }
 
 // np.gradient(x, 2, edge_order=2) at index i of a line of n samples with stride st
-__device__ __forceinline__ float gradient2(const float* x, int i, int n, int st) {
+// x holds the samples lo, lo + 1, ... of the line (lo = 0: the whole line); every index read must be >= lo
+__device__ __forceinline__ float gradient2(const float* x, int i, int n, int st, int lo = 0) {
+  auto at = [&](int j) { return x[(size_t)(j - lo) * st]; };
   if (i == 0)
-    return __fadd_rn(__fadd_rn(__fmul_rn(-0.75f, x[0]), x[st]), __fmul_rn(-0.25f, x[2 * st]));
+    return __fadd_rn(__fadd_rn(__fmul_rn(-0.75f, at(0)), at(1)), __fmul_rn(-0.25f, at(2)));
   if (i == n - 1)
-    return __fadd_rn(__fadd_rn(__fmul_rn(0.25f, x[(size_t)(n - 3) * st]), -x[(size_t)(n - 2) * st]),
-                     __fmul_rn(0.75f, x[(size_t)(n - 1) * st]));
-  return __fdiv_rn(__fsub_rn(x[(size_t)(i + 1) * st], x[(size_t)(i - 1) * st]), 4.f);
+    return __fadd_rn(__fadd_rn(__fmul_rn(0.25f, at(n - 3)), -at(n - 2)), __fmul_rn(0.75f, at(n - 1)));
+  return __fdiv_rn(__fsub_rn(at(i + 1), at(i - 1)), 4.f);
 }
 
-__global__ void __launch_bounds__(kScene)
-normals_kernel(int H, int W, const float* __restrict__ depth, const float* __restrict__ Kmat, float lo, float hi,
-               const float* __restrict__ S, float* __restrict__ map) {
-  const size_t plane = (size_t)H * W;
-  const int pix = blockIdx.x * kScene + threadIdx.x, f = blockIdx.y;
-  if (pix >= H * W) return;
-  const int v = pix / W, u = pix - v * W;
-  const float* K = Kmat + 9 * f;
+// stage 1's map entry m[0..6) of pixel (u, v): smoothed depth z and its gradients gu, gv; raw depth d
+__device__ __forceinline__ void map_entry(int u, int v, const float* K, float z, float gu, float gv, float d, float lo,
+                                          float hi, float* m) {
   const float fx = K[0], cx = K[2], fy = K[4], cy = K[5];
-  const float* s = S + f * plane;
-  const float z = s[pix];
-  const float gv = gradient2(s + u, v, H, W), gu = gradient2(s + (size_t)v * W, u, W, 1);
   const float a = __fsub_rn((float)u, cx), b = __fsub_rn((float)v, cy);
   const float ix = __frcp_rn(fx), iy = __frcp_rn(fy);
   const float tux = __fadd_rn(__fmul_rn(z, ix), __fmul_rn(__fmul_rn(a, ix), gu));
@@ -150,13 +176,106 @@ normals_kernel(int H, int W, const float* __restrict__ depth, const float* __res
   const float nn = __fsqrt_rn(__fadd_rn(__fadd_rn(__fmul_rn(nx, nx), __fmul_rn(ny, ny)), __fmul_rn(nz, nz)));
   if (nn > 0.f) { nx = __fdiv_rn(nx, nn); ny = __fdiv_rn(ny, nn); nz = __fdiv_rn(nz, nn); }
   else { nx = ny = nz = 0.f; }
-  const float d = depth[f * plane + pix];
   const bool ok = d > lo && d < hi;
-  float* m = map + (f * plane + pix) * 6;
   m[0] = ok ? __fdiv_rn(__fmul_rn(a, d), fx) : 0.f;
   m[1] = ok ? __fdiv_rn(__fmul_rn(b, d), fy) : 0.f;
   m[2] = ok ? d : 0.f;
   m[3] = nx; m[4] = ny; m[5] = nz;
+}
+
+__global__ void __launch_bounds__(kScene)
+normals_kernel(int H, int W, const float* __restrict__ depth, const float* __restrict__ Kmat, float lo, float hi,
+               const float* __restrict__ S, float* __restrict__ map) {
+  const size_t plane = (size_t)H * W;
+  const int pix = blockIdx.x * kScene + threadIdx.x, f = blockIdx.y;
+  if (pix >= H * W) return;
+  const int v = pix / W, u = pix - v * W;
+  const float* s = S + f * plane;
+  const float gv = gradient2(s + u, v, H, W), gu = gradient2(s + (size_t)v * W, u, W, 1);
+  map_entry(u, v, Kmat + 9 * f, s[pix], gu, gv, depth[f * plane + pix], lo, hi, map + (f * plane + pix) * 6);
+}
+
+// ---- masked normals (1'): one grid row per detection, box- or ext-relative pixel t of a tile
+__device__ __forceinline__ bool in_box(const int* b, int u, int v) { return u >= b[0] && u < b[2] && v >= b[1] && v < b[3]; }
+
+__global__ void __launch_bounds__(kScene)
+mask_tiles_kernel(int H, int W, const MaskDet* __restrict__ dets, const uint8_t* __restrict__ dense,
+                  const long long* __restrict__ ends, uint8_t* __restrict__ tiles) {
+  const MaskDet& dt = dets[blockIdx.y];
+  const int bw = dt.box[2] - dt.box[0], bh = dt.box[3] - dt.box[1];
+  const int t = blockIdx.x * kScene + threadIdx.x;
+  if (bw <= 0 || bh <= 0 || t >= bw * bh) return;
+  const int v = dt.box[1] + t / bw, u = dt.box[0] + t % bw;
+  const bool m = dense ? dense[(size_t)blockIdx.y * H * W + (size_t)v * W + u] != 0
+                       : gp::rle_bit(ends, dt.run0, dt.run1, (long long)u * H + v);          // column-major runs
+  tiles[dt.tile + t] = m;
+}
+
+// pass 1, along v, over the ext tile: num = sum w D [D > 0] M, den = sum w [D > 0] M (M = 0 outside the box)
+__global__ void __launch_bounds__(kScene)
+masked_smooth_v_kernel(int H, int W, const MaskDet* __restrict__ dets, const float* __restrict__ depth,
+                       const uint8_t* __restrict__ tiles, float* __restrict__ num, float* __restrict__ den) {
+  __shared__ float w[2 * kRadius + 1];
+  if (threadIdx.x == 0) gauss_weights(w);
+  __syncthreads();
+  const MaskDet& dt = dets[blockIdx.y];
+  const int ew = dt.ext[2] - dt.ext[0], eh = dt.ext[3] - dt.ext[1], bw = dt.box[2] - dt.box[0];
+  const int t = blockIdx.x * kScene + threadIdx.x;
+  if (ew <= 0 || eh <= 0 || t >= ew * eh) return;
+  const int v = dt.ext[1] + t / ew, u = dt.ext[0] + t % ew;
+  const float* d = depth + (size_t)dt.frame * H * W;
+  const uint8_t* m = tiles + dt.tile;
+  float sn = 0.f, sd = 0.f;
+  for (int k = -kRadius; k <= kRadius; ++k) {
+    const int r = reflect(v + k, H);
+    if (!in_box(dt.box, u, r) || !m[(size_t)(r - dt.box[1]) * bw + (u - dt.box[0])]) continue;
+    const float z = d[(size_t)r * W + u];
+    if (z > 0.f) { sn = __fadd_rn(sn, __fmul_rn(w[k + kRadius], z)); sd = __fadd_rn(sd, w[k + kRadius]); }
+  }
+  num[dt.ext_off + t] = sn;
+  den[dt.ext_off + t] = sd;
+}
+
+// pass 2, along u: S = (G_u * num) / (G_u * den); columns outside the ext tile hold num = den = 0 and add +0
+__global__ void __launch_bounds__(kScene)
+masked_smooth_u_kernel(int W, const MaskDet* __restrict__ dets, const float* __restrict__ num,
+                       const float* __restrict__ den, float* __restrict__ S) {
+  __shared__ float w[2 * kRadius + 1];
+  if (threadIdx.x == 0) gauss_weights(w);
+  __syncthreads();
+  const MaskDet& dt = dets[blockIdx.y];
+  const int ew = dt.ext[2] - dt.ext[0], eh = dt.ext[3] - dt.ext[1];
+  const int t = blockIdx.x * kScene + threadIdx.x;
+  if (ew <= 0 || eh <= 0 || t >= ew * eh) return;
+  const int row = t / ew, u = dt.ext[0] + t % ew;
+  const float* a = num + dt.ext_off + (size_t)row * ew;
+  const float* b = den + dt.ext_off + (size_t)row * ew;
+  float sn = 0.f, sd = 0.f;
+  for (int k = -kRadius; k <= kRadius; ++k) {
+    const int j = reflect(u + k, W);
+    if (j < dt.ext[0] || j >= dt.ext[2]) continue;
+    sn = __fadd_rn(sn, __fmul_rn(w[k + kRadius], a[j - dt.ext[0]]));
+    sd = __fadd_rn(sd, __fmul_rn(w[k + kRadius], b[j - dt.ext[0]]));
+  }
+  S[dt.ext_off + t] = sd > 0.f ? __fdiv_rn(sn, sd) : 0.f;
+}
+
+// the map over the box: gradients of the ext tile at frame indices (stencils stay inside ext by kMargin)
+__global__ void __launch_bounds__(kScene)
+masked_normals_kernel(int H, int W, const MaskDet* __restrict__ dets, const float* __restrict__ depth,
+                      const float* __restrict__ Kmat, float lo, float hi, const float* __restrict__ S,
+                      float* __restrict__ map) {
+  const MaskDet& dt = dets[blockIdx.y];
+  const int bw = dt.box[2] - dt.box[0], bh = dt.box[3] - dt.box[1], ew = dt.ext[2] - dt.ext[0];
+  const int t = blockIdx.x * kScene + threadIdx.x;
+  if (bw <= 0 || bh <= 0 || t >= bw * bh) return;
+  const int v = dt.box[1] + t / bw, u = dt.box[0] + t % bw;
+  const float* s = S + dt.ext_off;
+  const float* col = s + (u - dt.ext[0]);                       // column u from frame row ext[1]
+  const float* row = s + (size_t)(v - dt.ext[1]) * ew;           // row v from frame column ext[0]
+  const float gv = gradient2(col, v, H, ew, dt.ext[1]), gu = gradient2(row, u, W, 1, dt.ext[0]);
+  map_entry(u, v, Kmat + 9 * dt.frame, row[u - dt.ext[0]], gu, gv, depth[(size_t)dt.frame * H * W + (size_t)v * W + u], lo, hi,
+            map + (dt.tile + t) * 6);
 }
 
 struct HypWork {   // per-hypothesis slices of the workspace, H * W entries each
@@ -275,12 +394,17 @@ __device__ __forceinline__ void rodrigues(const double w[3], double R[9]) {
   R[6] = -A * y + B * x * z;        R[7] = A * x + B * y * z;     R[8] = 1.0 - B * (x * x + y * y);
 }
 
+// kBox = false: frame maps [n_frames,H,W,6], frame_idx [n_hyp] and optional full-frame masks [n_hyp,H,W] (stages 1-2).
+// kBox = true: the masked mode (1'-2'): frame_idx is det_idx [n_hyp] into the n_frames entries of `dets`, the map and
+// mask are the detection's box tiles, and the per-hypothesis scratch holds `scratch` entries (>= every box area).
+template <bool kBox>
 __global__ void __launch_bounds__(kThreads, 1)
 icp_kernel(int n_frames, int H, int W, const int32_t* __restrict__ frame_idx, const uint8_t* __restrict__ masks,
            const float* __restrict__ rendered, const int64_t* __restrict__ boxes, const float* __restrict__ T0,
            const float* __restrict__ Kmat, const float* __restrict__ map, gp_icp_params_t p, int* src_all,
            unsigned* dist_all, int* tgt_all, float* __restrict__ out_pose, int32_t* __restrict__ out_status,
-           float* __restrict__ out_residual, float* __restrict__ out_fitness) {
+           float* __restrict__ out_residual, float* __restrict__ out_fitness, const MaskDet* __restrict__ dets,
+           long long scratch) {
   __shared__ Shared sh;
   const int h = blockIdx.x, tid = threadIdx.x;
   const size_t plane = (size_t)H * W;
@@ -294,13 +418,26 @@ icp_kernel(int n_frames, int H, int W, const int32_t* __restrict__ frame_idx, co
     if (tid < 16) po[tid] = t0[tid];
     if (tid == 0) { out_status[h] = status; out_residual[h] = res; out_fitness[h] = fit; }
   };
-  const int f = frame_idx[h];
-  if (f < 0 || f >= n_frames) { keep_T0(GP_ICP_INVALID, -1.f, 0.f); return; }
-  HypWork wk{src_all + h * plane, dist_all + h * plane, tgt_all + h * plane};
+  const int fi = frame_idx[h];
+  if (fi < 0 || fi >= n_frames) { keep_T0(GP_ICP_INVALID, -1.f, 0.f); return; }
+  // target region: the frame, or the mask box (tb) with box-relative map and mask tiles
+  int tb[4] = {0, 0, W, H};
+  if (kBox) {
+    for (int k = 0; k < 4; ++k) tb[k] = dets[fi].box[k];
+    if (tb[2] < tb[0]) tb[2] = tb[0];
+    if (tb[3] < tb[1]) tb[3] = tb[1];
+    if ((long long)(tb[2] - tb[0]) * (tb[3] - tb[1]) > scratch) { keep_T0(GP_ICP_INVALID, -1.f, 0.f); return; }
+  }
+  const int f = kBox ? dets[fi].frame : fi, tw = tb[2] - tb[0];
+  const size_t stride = kBox ? (size_t)scratch : plane;
+  HypWork wk{src_all + h * stride, dist_all + h * stride, tgt_all + h * stride};
   const float* R = rendered + h * plane;
-  const float* M = map + f * plane * 6;
-  const uint8_t* mask = masks ? masks + h * plane : nullptr;
+  const float* M = kBox ? map + dets[fi].tile * 6 : map + f * plane * 6;
+  const uint8_t* mask = kBox ? masks + dets[fi].tile : masks ? masks + h * plane : nullptr;
   const float delta = __fmul_rn(0.1f, upm);
+  auto entry = [&](int u, int v) -> size_t {          // map / mask entry of frame pixel (u, v) inside tb
+    return kBox ? (size_t)(v - tb[1]) * tw + (u - tb[0]) : (size_t)v * W + u;
+  };
   if (tid == 0) {
     const float* K = Kmat + 9 * f;
     sh.K[0] = K[0]; sh.K[1] = K[4]; sh.K[2] = K[2]; sh.K[3] = K[5];
@@ -310,17 +447,19 @@ icp_kernel(int n_frames, int H, int W, const int32_t* __restrict__ frame_idx, co
   }
   __syncthreads();
   const float fx = sh.K[0], fy = sh.K[1], cx = sh.K[2], cy = sh.K[3];
-  auto target_ok = [&](size_t q) -> bool {
-    const float d = M[q * 6 + 2];
+  auto target_ok = [&](int u, int v) -> bool {
+    const size_t e = entry(u, v);
+    const float d = M[e * 6 + 2];
     if (!(d > 0.f)) return false;
-    if (mask) return mask[q] != 0;
-    const float r = R[q];
+    if (mask) return mask[e] != 0;
+    const float r = R[(size_t)v * W + u];
     return r > 0.f && fabsf(__fsub_rn(d, r)) <= delta;
   };
 
   // stages 2-4: counts and centroids of both sets, sources compacted in row-major order inside the box
   const int bx0 = sh.box[0], by0 = sh.box[1], bw = sh.box[2] - sh.box[0], bh = sh.box[3] - sh.box[1];
-  const int rx0 = mask ? 0 : bx0, ry0 = mask ? 0 : by0, rw = mask ? W : max(bw, 0), rh = mask ? H : max(bh, 0);
+  const int rx0 = mask ? tb[0] : bx0, ry0 = mask ? tb[1] : by0, rw = mask ? tw : max(bw, 0);
+  const int rh = mask ? tb[3] - tb[1] : max(bh, 0);
   double acc[7] = {0, 0, 0, 0, 0, 0, 0};            // targets: n, x, y, z; sources: x, y, z
   int nsrc = 0;
   const int region = rw * rh;
@@ -329,9 +468,9 @@ icp_kernel(int n_frames, int H, int W, const int32_t* __restrict__ frame_idx, co
     bool is_src = false;
     if (i < region) {
       const int v = ry0 + i / rw, u = rx0 + i % rw;
-      const size_t q = (size_t)v * W + u;
-      if (target_ok(q)) {
-        acc[0] += 1.0; acc[1] += M[q * 6]; acc[2] += M[q * 6 + 1]; acc[3] += M[q * 6 + 2];
+      const size_t q = (size_t)v * W + u, e = entry(u, v);
+      if (target_ok(u, v)) {
+        acc[0] += 1.0; acc[1] += M[e * 6]; acc[2] += M[e * 6 + 1]; acc[3] += M[e * 6 + 2];
         const float r = R[q];
         if (r > 0.f && u >= bx0 && u < bx0 + bw && v >= by0 && v < by0 + bh) {
           is_src = true;
@@ -393,15 +532,15 @@ icp_kernel(int n_frames, int H, int W, const int32_t* __restrict__ frame_idx, co
           const float pv = __fadd_rn(__fdiv_rn(__fmul_rn(fy, s[1]), s[2]), cy);
           if (fabsf(pu) < 1e7f && fabsf(pv) < 1e7f) {
             const int cu = (int)rintf(pu), cv = (int)rintf(pv);
-            const int u0 = max(cu - rad, 0), u1 = min(cu + rad, W - 1);
-            const int v0 = max(cv - rad, 0), v1 = min(cv + rad, H - 1);
+            const int u0 = max(cu - rad, tb[0]), u1 = min(cu + rad, tb[2] - 1);
+            const int v0 = max(cv - rad, tb[1]), v1 = min(cv + rad, tb[3] - 1);
             float bd = 0.f;
             for (int vv = v0; vv <= v1; ++vv)
               for (int uu = u0; uu <= u1; ++uu) {
-                const size_t t = (size_t)vv * W + uu;
-                if (!target_ok(t)) continue;
-                const float dx = __fsub_rn(M[t * 6], s[0]), dy = __fsub_rn(M[t * 6 + 1], s[1]);
-                const float dz = __fsub_rn(M[t * 6 + 2], s[2]);
+                if (!target_ok(uu, vv)) continue;
+                const size_t t = (size_t)vv * W + uu, e = entry(uu, vv);
+                const float dx = __fsub_rn(M[e * 6], s[0]), dy = __fsub_rn(M[e * 6 + 1], s[1]);
+                const float dz = __fsub_rn(M[e * 6 + 2], s[2]);
                 const float d2 = __fadd_rn(__fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy)), __fmul_rn(dz, dz));
                 if (bi < 0 || d2 < bd) { bd = d2; bi = (int)t; }
               }
@@ -450,7 +589,7 @@ icp_kernel(int n_frames, int H, int W, const int32_t* __restrict__ frame_idx, co
         for (int r = 0; r < 3; ++r)
           s[r] = __fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(T[4 * r], x), __fmul_rn(T[4 * r + 1], y)),
                                      __fmul_rn(T[4 * r + 2], z)), T[4 * r + 3]);
-        const float* tm = M + (size_t)t * 6;
+        const float* tm = M + (kBox ? entry(t % W, t / W) : (size_t)t) * 6;
         const double nx = tm[3], ny = tm[4], nz = tm[5];
         const double r = (s[0] - tm[0]) * nx + (s[1] - tm[1]) * ny + (s[2] - tm[2]) * nz;
         const double j[6] = {(s[1] * nz - s[2] * ny) / L, (s[2] * nx - s[0] * nz) / L, (s[0] * ny - s[1] * nx) / L,
@@ -574,7 +713,178 @@ int check_sizes(int n_frames, int n_hyp, int H, int W) {
   return GP_OK;
 }
 
+int check_params(const gp_icp_params_t* params) {
+  if (!params) return fail(GP_ERR_INVALID, "null params");
+  const gp_icp_params_t& p = *params;
+  if (!(p.unit_per_m > 0.f) || !isfinite(p.unit_per_m))
+    return fail(GP_ERR_INVALID, "unit_per_m must be positive and finite");
+  if (p.min_points < 1) return fail(GP_ERR_INVALID, "min_points %d must be >= 1", p.min_points);
+  if (p.num_levels < 1 || p.num_levels > kMaxLevels)
+    return fail(GP_ERR_INVALID, "num_levels %d outside [1, %d]", p.num_levels, kMaxLevels);
+  if (p.max_iters < 1 || p.max_iters > 100000) return fail(GP_ERR_INVALID, "max_iters %d outside [1, 100000]", p.max_iters);
+  if (!(p.rejection_scale > 0.f) || !isfinite(p.rejection_scale))
+    return fail(GP_ERR_INVALID, "rejection_scale must be positive and finite");
+  if (!(p.max_residual >= 0.f) || !(p.min_step_rad >= 0.f) || !(p.min_step_m >= 0.f))
+    return fail(GP_ERR_INVALID, "max_residual, min_step_rad and min_step_m must be >= 0");
+  if (p.debug.trace && (p.debug.trace_capacity < 1 || !p.debug.trace_count))
+    return fail(GP_ERR_INVALID, "debug.trace needs trace_capacity >= 1 and trace_count");
+  return GP_OK;
+}
+
+// the masked workspace: the detection table, then the mask tiles, the map, num, den, S and the run ends
+struct MaskLayout {
+  std::vector<MaskDet> dets;
+  long long tiles = 0, exts = 0, box_max = 0, ext_max = 0, runs = 0;
+  size_t table_b = 0, tiles_b = 0, map_b = 0, ext_b = 0, ends_b = 0;
+  size_t bytes() const { return table_b + tiles_b + map_b + 3 * ext_b + ends_b; }
+};
+
+int mask_layout(int n_frames, int H, int W, const gp_icp_mask_set_t* set, MaskLayout* L) {
+  if (const int rc = check_sizes(n_frames, 0, H, W)) return rc;
+  if (!set) return fail(GP_ERR_INVALID, "null mask set");
+  const int n = set->n_det;
+  if (n < 0 || n > 65535) return fail(GP_ERR_INVALID, "n_det %d outside [0, 65535]", n);
+  if (n && (!set->frame || !set->boxes)) return fail(GP_ERR_INVALID, "null frame / boxes");
+  const int64_t* ro = set->run_offsets;
+  if (ro && ro[0] < 0) return fail(GP_ERR_INVALID, "run_offsets[0] = %lld is negative", (long long)ro[0]);
+  L->dets.resize(n);
+  for (int d = 0; d < n; ++d) {
+    const int32_t* b = set->boxes + 4 * (size_t)d;
+    if (set->frame[d] < 0 || set->frame[d] >= n_frames)
+      return fail(GP_ERR_INVALID, "frame[%d] = %d outside [0, %d)", d, set->frame[d], n_frames);
+    if (b[0] < 0 || b[0] > b[2] || b[2] > W || b[1] < 0 || b[1] > b[3] || b[3] > H)
+      return fail(GP_ERR_INVALID, "box %d (%d, %d, %d, %d) is not 0 <= x0 <= x1 <= %d, 0 <= y0 <= y1 <= %d", d, b[0],
+                  b[1], b[2], b[3], W, H);
+    if (ro && ro[d + 1] < ro[d])
+      return fail(GP_ERR_INVALID, "run_offsets decrease at detection %d (%lld -> %lld)", d, (long long)ro[d],
+                  (long long)ro[d + 1]);
+    MaskDet& m = L->dets[d];
+    const bool empty = b[0] == b[2] || b[1] == b[3];
+    for (int k = 0; k < 4; ++k) m.box[k] = b[k];
+    m.ext[0] = empty ? b[0] : max(0, b[0] - kMargin); m.ext[1] = empty ? b[1] : max(0, b[1] - kMargin);
+    m.ext[2] = empty ? b[0] : min(W, b[2] + kMargin); m.ext[3] = empty ? b[1] : min(H, b[3] + kMargin);
+    m.frame = set->frame[d];
+    m.reserved = 0;
+    m.tile = L->tiles;
+    m.ext_off = L->exts;
+    m.run0 = ro ? ro[d] : 0;
+    m.run1 = ro ? ro[d + 1] : 0;
+    const long long area = (long long)(b[2] - b[0]) * (b[3] - b[1]);
+    const long long ext = (long long)(m.ext[2] - m.ext[0]) * (m.ext[3] - m.ext[1]);
+    L->tiles += area;
+    L->exts += ext;
+    L->box_max = std::max(L->box_max, area);
+    L->ext_max = std::max(L->ext_max, ext);
+  }
+  L->runs = ro ? ro[n] : 0;
+  L->table_b = align256((size_t)n * sizeof(MaskDet));
+  L->tiles_b = align256((size_t)L->tiles);
+  L->map_b = align256((size_t)L->tiles * 6 * sizeof(float));
+  L->ext_b = align256((size_t)L->exts * sizeof(float));
+  L->ends_b = align256((size_t)L->runs * sizeof(long long));
+  return GP_OK;
+}
+
+struct MaskPtrs {
+  MaskDet* dets;
+  uint8_t* tiles;
+  float *map, *num, *den, *S;
+  long long* ends;
+};
+
+MaskPtrs mask_ptrs(const MaskLayout& L, void* workspace) {
+  char* w = static_cast<char*>(workspace);
+  MaskPtrs p;
+  p.dets = reinterpret_cast<MaskDet*>(w);
+  p.tiles = reinterpret_cast<uint8_t*>(w += L.table_b);
+  p.map = reinterpret_cast<float*>(w += L.tiles_b);
+  p.num = reinterpret_cast<float*>(w += L.map_b);
+  p.den = reinterpret_cast<float*>(w += L.ext_b);
+  p.S = reinterpret_cast<float*>(w += L.ext_b);
+  p.ends = reinterpret_cast<long long*>(w += L.ext_b);
+  return p;
+}
+
+unsigned blocks(long long pixels) { return (unsigned)((pixels + kScene - 1) / kScene); }
+
 }  // namespace
+
+extern "C" int gp_icp_masked_query_sizes(int n_frames, int height, int width, const gp_icp_mask_set_t* set,
+                                         size_t* workspace_bytes, int64_t* box_pixels, size_t* tiles_offset,
+                                         size_t* map_offset) {
+  MaskLayout L;
+  if (const int rc = mask_layout(n_frames, height, width, set, &L)) return rc;
+  if (!workspace_bytes || !box_pixels) return fail(GP_ERR_INVALID, "null workspace_bytes / box_pixels");
+  *workspace_bytes = L.bytes();
+  *box_pixels = L.box_max;
+  if (tiles_offset) *tiles_offset = L.table_b;
+  if (map_offset) *map_offset = L.table_b + L.tiles_b;
+  return GP_OK;
+}
+
+extern "C" int gp_icp_masked_decode(int n_frames, int height, int width, const gp_icp_mask_set_t* set,
+                                    const uint8_t* masks, const int32_t* counts, void* workspace, void* stream) {
+  MaskLayout L;
+  if (const int rc = mask_layout(n_frames, height, width, set, &L)) return rc;
+  if (!workspace) return fail(GP_ERR_INVALID, "null workspace");
+  if (!masks == !set->run_offsets) return fail(GP_ERR_INVALID, "give either dense masks or run_offsets, not both");
+  if (!masks && L.runs > 0 && !counts) return fail(GP_ERR_INVALID, "null counts");
+  const int n = set->n_det;
+  if (n == 0) return GP_OK;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const MaskPtrs P = mask_ptrs(L, workspace);
+  GP_CUDA(cudaMemcpyAsync(P.dets, L.dets.data(), (size_t)n * sizeof(MaskDet), cudaMemcpyHostToDevice, st));
+  if (!masks && L.runs > 0) GP_CUDA(gp::launch_rle_scan(n, counts, set->run_offsets, P.ends, st));
+  if (L.box_max > 0)
+    GP_CUDA(gp::launch_ex(mask_tiles_kernel, dim3(blocks(L.box_max), n), kScene, 0, st, 1, false, height, width,
+                          P.dets, masks, P.ends, P.tiles));
+  return GP_OK;
+}
+
+extern "C" int gp_icp_prepare_masked_scene(int n_frames, int height, int width, const gp_icp_mask_set_t* set,
+                                           const float* depth, const float* K, float unit_per_m, void* workspace,
+                                           void* stream) {
+  MaskLayout L;
+  if (const int rc = mask_layout(n_frames, height, width, set, &L)) return rc;
+  if (!depth || !K || !workspace) return fail(GP_ERR_INVALID, "null argument");
+  if (!(unit_per_m > 0.f) || !isfinite(unit_per_m))
+    return fail(GP_ERR_INVALID, "unit_per_m must be positive and finite");
+  const int n = set->n_det;
+  if (n == 0 || L.box_max == 0) return GP_OK;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const MaskPtrs P = mask_ptrs(L, workspace);
+  const dim3 ge(blocks(L.ext_max), n), gb(blocks(L.box_max), n);
+  GP_CUDA(gp::launch_ex(masked_smooth_v_kernel, ge, kScene, 0, st, 1, false, height, width, P.dets, depth, P.tiles,
+                        P.num, P.den));
+  GP_CUDA(gp::launch_ex(masked_smooth_u_kernel, ge, kScene, 0, st, 1, false, width, P.dets, P.num, P.den, P.S));
+  GP_CUDA(gp::launch_ex(masked_normals_kernel, gb, kScene, 0, st, 1, false, height, width, P.dets, depth, K,
+                        0.2f * unit_per_m, 5.f * unit_per_m, P.S, P.map));
+  return GP_OK;
+}
+
+extern "C" int gp_icp_refine_masked(int n_frames, int height, int width, const gp_icp_mask_set_t* set, int n_hyp,
+                                    const int32_t* det_idx, const float* rendered_depth, const int64_t* boxes,
+                                    const float* T0, const float* K, const gp_icp_params_t* params, float* out_poses,
+                                    int32_t* out_status, float* out_residual, float* out_fitness,
+                                    const void* scene_workspace, void* workspace, void* stream) {
+  MaskLayout L;
+  if (const int rc = mask_layout(n_frames, height, width, set, &L)) return rc;
+  if (const int rc = check_sizes(n_frames, n_hyp, height, width)) return rc;
+  if (const int rc = check_params(params)) return rc;
+  if (!det_idx || !rendered_depth || !boxes || !T0 || !K || !out_poses || !out_status || !out_residual ||
+      !out_fitness || !scene_workspace || (!workspace && L.box_max > 0))
+    return fail(GP_ERR_INVALID, "null argument");
+  if (n_hyp == 0) return GP_OK;
+  const size_t per = (size_t)n_hyp * L.box_max;
+  int* src = static_cast<int*>(workspace);
+  unsigned* dist = reinterpret_cast<unsigned*>(src + per);
+  int* tgt = reinterpret_cast<int*>(dist + per);
+  const MaskPtrs P = mask_ptrs(L, const_cast<void*>(scene_workspace));
+  GP_CUDA(gp::launch_ex(icp_kernel<true>, n_hyp, kThreads, 0, static_cast<cudaStream_t>(stream), 1, false, set->n_det,
+                        height, width, det_idx, P.tiles, rendered_depth, boxes, T0, K, P.map, *params, src, dist, tgt,
+                        out_poses, out_status, out_residual, out_fitness, P.dets, L.box_max));
+  return GP_OK;
+}
 
 extern "C" int gp_icp_query_sizes(int n_frames, int n_hyp, int height, int width, size_t* workspace_bytes) {
   if (const int rc = check_sizes(n_frames, n_hyp, height, width)) return rc;
@@ -608,23 +918,11 @@ extern "C" int gp_icp_refine(int n_frames, int n_hyp, int height, int width, con
                              const float* K, const gp_icp_params_t* params, float* out_poses, int32_t* out_status,
                              float* out_residual, float* out_fitness, void* workspace, void* stream) {
   if (const int rc = check_sizes(n_frames, n_hyp, height, width)) return rc;
-  if (!params) return fail(GP_ERR_INVALID, "null params");
+  if (const int rc = check_params(params)) return rc;
   const gp_icp_params_t& p = *params;
-  if (!(p.unit_per_m > 0.f) || !isfinite(p.unit_per_m))
-    return fail(GP_ERR_INVALID, "unit_per_m must be positive and finite");
-  if (p.min_points < 1) return fail(GP_ERR_INVALID, "min_points %d must be >= 1", p.min_points);
-  if (p.num_levels < 1 || p.num_levels > kMaxLevels)
-    return fail(GP_ERR_INVALID, "num_levels %d outside [1, %d]", p.num_levels, kMaxLevels);
-  if (p.max_iters < 1 || p.max_iters > 100000) return fail(GP_ERR_INVALID, "max_iters %d outside [1, 100000]", p.max_iters);
-  if (!(p.rejection_scale > 0.f) || !isfinite(p.rejection_scale))
-    return fail(GP_ERR_INVALID, "rejection_scale must be positive and finite");
-  if (!(p.max_residual >= 0.f) || !(p.min_step_rad >= 0.f) || !(p.min_step_m >= 0.f))
-    return fail(GP_ERR_INVALID, "max_residual, min_step_rad and min_step_m must be >= 0");
   if (!frame_idx || !rendered_depth || !boxes || !T0 || !K || !out_poses || !out_status || !out_residual ||
       !out_fitness || !workspace)
     return fail(GP_ERR_INVALID, "null argument");
-  if (p.debug.trace && (p.debug.trace_capacity < 1 || !p.debug.trace_count))
-    return fail(GP_ERR_INVALID, "debug.trace needs trace_capacity >= 1 and trace_count");
   if (n_hyp == 0) return GP_OK;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const size_t plane = (size_t)height * width;
@@ -633,9 +931,9 @@ extern "C" int gp_icp_refine(int n_frames, int n_hyp, int height, int width, con
   int* src = reinterpret_cast<int*>(ws + scene_bytes(n_frames, height, width));
   unsigned* dist = reinterpret_cast<unsigned*>(src + n_hyp * plane);
   int* tgt = reinterpret_cast<int*>(dist + n_hyp * plane);
-  GP_CUDA(gp::launch_ex(icp_kernel, n_hyp, kThreads, 0, st, 1, false, n_frames, height, width, frame_idx, masks,
+  GP_CUDA(gp::launch_ex(icp_kernel<false>, n_hyp, kThreads, 0, st, 1, false, n_frames, height, width, frame_idx, masks,
                         rendered_depth, boxes, T0, K, map, p, src, dist, tgt, out_poses, out_status, out_residual,
-                        out_fitness));
+                        out_fitness, nullptr, 0LL));
   return GP_OK;
 }
 

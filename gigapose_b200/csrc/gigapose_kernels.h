@@ -204,4 +204,21 @@ cudaError_t launch_attention_tc(const CUtensorMap& hi128, const CUtensorMap& lo1
 cudaError_t read_attention_stamps(long long* host32);
 cudaError_t read_gemm_stamps(long long* host128);
 
+// ---------------------------------------------------------------- COCO run-length masks (preprocess.cu)
+// ends[k] = counts[offsets[i]] + ... + counts[k] over the runs of each of the n detections; offsets [n+1] is host
+// memory.  One CTA per detection, in launches of up to 256 detections.
+cudaError_t launch_rle_scan(int n, const int32_t* counts, const int64_t* offsets, long long* ends, cudaStream_t s);
+
+// The mask value at column-major run position p of a detection whose running sums are ends[r0 .. r1): the parity of the
+// first run whose end lies past p (odd runs are ones); past the last run, 0.
+__device__ __forceinline__ bool rle_bit(const long long* __restrict__ ends, long long r0, long long r1, long long p) {
+  long long lo = r0, hi = r1;
+  while (lo < hi) {
+    const long long mid = (lo + hi) >> 1;
+    if (ends[mid] <= p) lo = mid + 1;
+    else hi = mid;
+  }
+  return lo < r1 && ((lo - r0) & 1);
+}
+
 }  // namespace gp

@@ -167,13 +167,7 @@ rle_scan_kernel(const int32_t* __restrict__ counts, RleOffsets ro, long long* __
 }
 
 __device__ __forceinline__ float rle_value(const long long* __restrict__ ends, long long r0, long long r1, long long p) {
-  long long lo = r0, hi = r1;                                          // first run whose end lies past p
-  while (lo < hi) {
-    const long long mid = (lo + hi) >> 1;
-    if (ends[mid] <= p) lo = mid + 1;
-    else hi = mid;
-  }
-  return lo < r1 && ((lo - r0) & 1) ? 1.f : 0.f;                       // odd runs are ones; past the last run, 0
+  return gp::rle_bit(ends, r0, r1, p) ? 1.f : 0.f;
 }
 
 __global__ void __launch_bounds__(256)
@@ -213,6 +207,16 @@ crop_resize_pad_rle_kernel(int H, int W, int T, int det_base, const uint8_t* __r
 }
 
 }  // namespace
+
+cudaError_t gp::launch_rle_scan(int n, const int32_t* counts, const int64_t* offsets, long long* ends, cudaStream_t s) {
+  for (int d0 = 0; d0 < n; d0 += kRleGroup) {
+    const int g = min(kRleGroup, n - d0);
+    RleOffsets ro;
+    for (int i = 0; i <= g; ++i) ro.off[i] = offsets[d0 + i];
+    if (const cudaError_t e = gp::launch_ex(rle_scan_kernel, dim3(g), 256, 0, s, 1, false, counts, ro, ends)) return e;
+  }
+  return cudaSuccess;
+}
 
 extern "C" int gp_crop_resize_pad(int n, int channels, int height, int width, int target_size, const float* images,
                                   const int32_t* image_index, const int64_t* xyxy_boxes, const float* mask, float in_div,

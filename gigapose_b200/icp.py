@@ -4,15 +4,17 @@
 (`gp_icp_refine`).  csrc/depth_icp.cu's header comment states the contract; it restates MegaPose's ICPRefiner
 (src/megapose/inference/icp_refiner.py:134-287) with the deviations listed in INTEGRATION.md.  Row f10:
 `score_hypotheses` renders final poses the same way and scores them against the measured depth (`gp_depth_score`,
-csrc/depth_score.cu), so that the best hypothesis of a detection can be kept."""
+csrc/depth_score.cu), so that the best hypothesis of a detection can be kept.  Row f11: `refine_icp_masked` smooths the
+target normals within each detection's own mask (dense or COCO run-length), over the mask's box only."""
 from __future__ import annotations
 
 import ctypes as C
 
+import numpy as np
 import torch
 
 from . import _lib
-from ._lib import GpIcpDebug, GpIcpParams, check, ptr
+from ._lib import GpIcpDebug, GpIcpMaskSet, GpIcpParams, check, ptr
 from .render import _device_mesh, render_chunk
 
 STATUS_NAMES = {_lib.ICP_OK: "ok", _lib.ICP_TOO_FEW_POINTS: "too few points", _lib.ICP_DEGENERATE: "degenerate",
@@ -197,3 +199,165 @@ def score_hypotheses(meshes_dev, labels, poses, depth, K, frame_idx, n_hyp, tole
                                          counts[sl].data_ptr(), score[sl].data_ptr(), best[s:e].data_ptr(),
                                          torch.cuda.current_stream(device).cuda_stream))
     return counts, score, best
+
+
+# ---------------------------------------------------------------------------------------------------- masked normals
+def rle_boxes(counts, offsets, H, W):
+    """Mask boxes i32 [n,4] (x0, y0, x1, y1, exclusive max; all 0 for an empty mask) of COCO run-length masks, from
+    the runs on the host: detection d owns counts[offsets[d]:offsets[d+1]], column-major, the first run counting
+    zeros; runs past H * W are cut off."""
+    counts = np.asarray(counts, np.int64).reshape(-1)
+    off = np.asarray(offsets, np.int64).reshape(-1)
+    out = np.zeros((len(off) - 1, 4), np.int32)
+    for d in range(len(off) - 1):
+        c = counts[off[d]:off[d + 1]]
+        ends = np.minimum(np.cumsum(c), H * W)
+        starts = np.minimum(ends - c, H * W)
+        ones = (np.arange(len(c)) % 2 == 1) & (ends > starts)
+        if not ones.any():
+            continue
+        s, e = starts[ones], ends[ones] - 1                            # first and last pixel of each run of ones
+        c0, c1 = s // H, e // H
+        r0 = np.where(c1 > c0, 0, s % H)                               # a run over two columns covers rows 0 .. H-1
+        r1 = np.where(c1 > c0, H - 1, e % H)
+        out[d] = (c0.min(), r0.min(), c1.max() + 1, r1.max() + 1)
+    return out
+
+
+def dense_boxes(masks):
+    """Mask boxes i32 [n,4] (as `rle_boxes`) of dense masks [n,H,W] (nonzero = in the mask), on the host."""
+    m = torch.as_tensor(masks) != 0
+    n, H, W = m.shape
+    rows, cols = m.any(2), m.any(1)
+    first = lambda a: a.to(torch.int8).argmax(1)                      # noqa: E731  (first True; 0 when none)
+    box = torch.stack([first(cols), first(rows), W - first(cols.flip(1)), H - first(rows.flip(1))], 1)
+    return torch.where(rows.any(1)[:, None], box, torch.zeros_like(box)).to("cpu", torch.int32).numpy()
+
+
+class MaskSet:
+    """The host description gp_icp_mask_set_t points to (frames, boxes, run offsets), kept alive with it."""
+
+    def __init__(self, frame, boxes, run_offsets=None):
+        self.frame = np.ascontiguousarray(np.asarray(frame).reshape(-1), np.int32)
+        self.boxes = np.ascontiguousarray(np.asarray(boxes).reshape(-1, 4), np.int32)
+        self.run_offsets = None if run_offsets is None else np.ascontiguousarray(np.asarray(run_offsets).reshape(-1),
+                                                                                 np.int64)
+        if self.boxes.shape[0] != self.frame.shape[0]:
+            raise ValueError("one box per detection")
+        if self.run_offsets is not None and self.run_offsets.shape[0] != self.frame.shape[0] + 1:
+            raise ValueError(f"run offsets need n_det + 1 = {self.frame.shape[0] + 1} entries")
+        i32 = C.POINTER(C.c_int32)
+        self.c = GpIcpMaskSet(len(self.frame), self.frame.ctypes.data_as(i32), self.boxes.ctypes.data_as(i32),
+                              None if self.run_offsets is None else self.run_offsets.ctypes.data_as(C.POINTER(C.c_int64)))
+
+    def __len__(self):
+        return len(self.frame)
+
+    def query(self, F, H, W, offsets=False):
+        """-> (scene workspace bytes, box_pixels), and with `offsets` the byte offsets of the tiles and the maps."""
+        b, px, t0, m0 = C.c_size_t(), C.c_int64(), C.c_size_t(), C.c_size_t()
+        check(_lib.load().gp_icp_masked_query_sizes(F, H, W, C.byref(self.c), C.byref(b), C.byref(px), C.byref(t0),
+                                                    C.byref(m0)))
+        return (b.value, px.value, t0.value, m0.value) if offsets else (b.value, px.value)
+
+    def tiles(self, workspace, F, H, W):
+        """Per detection, views (mask u8 [h,w], map f32 [h,w,6]) of its box in a decoded and prepared workspace."""
+        area = (self.boxes[:, 2] - self.boxes[:, 0]).astype(np.int64) * (self.boxes[:, 3] - self.boxes[:, 1])
+        start = np.concatenate([[0], np.cumsum(area)])
+        _, _, t0, m0 = self.query(F, H, W, offsets=True)
+        maps = workspace[m0:m0 + int(start[-1]) * 24].view(torch.float32)
+        out = []
+        for d, (x0, y0, x1, y1) in enumerate(self.boxes.tolist()):
+            h, w = max(y1 - y0, 0), max(x1 - x0, 0)
+            a, b = int(start[d]), int(start[d + 1])
+            out.append((workspace[t0 + a:t0 + b].reshape(h, w), maps[6 * a:6 * b].reshape(h, w, 6)))
+        return out
+
+
+def masked_scene(depth, K, det_frame, masks=None, rle=None, unit_per_m=1000.0):
+    """Decodes the detections' masks into box tiles and prepares their masked target maps (gp_icp_masked_decode +
+    gp_icp_prepare_masked_scene).  depth f32 [F,H,W] and K f32 [F,3,3] on the device, det_frame [n_det] frame of each
+    detection; masks dense [n_det,H,W] (device) or rle = (counts i32, offsets [n_det+1]) (host or device counts, host
+    offsets).  -> (workspace u8, MaskSet, box_pixels)."""
+    F, H, W = depth.shape
+    dev = depth.device
+    if (masks is None) == (rle is None):
+        raise ValueError("give either dense masks or rle = (counts, offsets)")
+    stream = torch.cuda.current_stream(dev).cuda_stream
+    n = len(np.asarray(det_frame).reshape(-1))
+    if masks is not None:
+        masks = torch.as_tensor(masks).to(dev)
+        if tuple(masks.shape) != (n, H, W):
+            raise ValueError(f"dense masks must be [{n},{H},{W}], got {tuple(masks.shape)}")
+        masks = (masks != 0).to(torch.uint8).contiguous()
+        ms, counts = MaskSet(det_frame, dense_boxes(masks)), None
+    else:
+        counts, off = rle
+        off = np.asarray(off, np.int64).reshape(-1)
+        counts = torch.as_tensor(np.asarray(counts) if not torch.is_tensor(counts) else counts,
+                                 dtype=torch.int32).reshape(-1)
+        if off.shape != (n + 1,) or counts.numel() < off[-1]:
+            raise ValueError(f"rle offsets must have n_det + 1 = {n + 1} entries within the {counts.numel()} counts")
+        ms = MaskSet(det_frame, rle_boxes(counts.cpu().numpy(), off, H, W), off)
+        counts = counts.to(dev, non_blocking=True).contiguous()
+    nbytes, box_pixels = ms.query(F, H, W)
+    ws = torch.empty(max(nbytes, 1), dtype=torch.uint8, device=dev)
+    lib = _lib.load()
+    check(lib.gp_icp_masked_decode(F, H, W, C.byref(ms.c), ptr(masks), ptr(counts), ws.data_ptr(), stream))
+    check(lib.gp_icp_prepare_masked_scene(F, H, W, C.byref(ms.c), depth.data_ptr(), K.data_ptr(), float(unit_per_m),
+                                          ws.data_ptr(), stream))
+    return ws, ms, box_pixels
+
+
+def refine_rendered_masked(ms, scene_ws, box_pixels, depth, K, det_idx, rendered, boxes, poses, debug=None, **params):
+    """gp_icp_refine_masked over n hypotheses against a prepared masked scene -> poses, status, residual, fitness."""
+    F, H, W = depth.shape
+    n = poses.shape[0]
+    dev = poses.device
+    out = torch.empty(n, 4, 4, device=dev)
+    status = torch.empty(n, dtype=torch.int32, device=dev)
+    residual = torch.empty(n, device=dev)
+    fitness = torch.empty(n, device=dev)
+    scratch = torch.empty(max(n * box_pixels * 12, 1), dtype=torch.uint8, device=dev)
+    p = make_params(debug, **params)
+    check(_lib.load().gp_icp_refine_masked(F, H, W, C.byref(ms.c), n, det_idx.data_ptr(), rendered.data_ptr(),
+                                           boxes.data_ptr(), poses.data_ptr(), K.data_ptr(), C.byref(p), out.data_ptr(),
+                                           status.data_ptr(), residual.data_ptr(), fitness.data_ptr(),
+                                           scene_ws.data_ptr(), scratch.data_ptr(),
+                                           torch.cuda.current_stream(dev).cuda_stream))
+    return out, status, residual, fitness
+
+
+@torch.no_grad()
+def refine_icp_masked(meshes_dev, labels, poses, depth, K, det_frame, det_idx, masks=None, rle=None, **params):
+    """`refine_icp` with target normals smoothed within each detection's mask (row f11, csrc/depth_icp.cu 1'-2').
+
+    det_frame [n_det] frame of each detection; det_idx [n] detection of each hypothesis (the hypotheses of a detection
+    share its map: no mask is copied per hypothesis); masks dense [n_det,H,W] or rle = (counts, offsets [n_det+1]) of
+    COCO run-length masks (bop_run's layout).  The rest as `refine_icp` -> (poses, status, residual, fitness)."""
+    upm = float(params.get("unit_per_m", DEFAULTS["unit_per_m"]))
+    det_frame = np.asarray(torch.as_tensor(det_frame).cpu(), np.int64).reshape(-1)
+    det_idx = np.asarray(torch.as_tensor(det_idx).cpu(), np.int64).reshape(-1)
+    if len(det_idx) and (det_idx.min() < 0 or det_idx.max() >= len(det_frame)):
+        raise ValueError(f"det_idx outside [0, {len(det_frame)})")
+    poses, depth, K, labels, frame_idx = _inputs("refine_icp_masked", meshes_dev, labels, poses, depth, K,
+                                                 det_frame[det_idx])
+    device = poses.device
+    F, H, W = depth.shape
+    n = poses.shape[0]
+    out = poses.clone()
+    status = torch.empty(n, dtype=torch.int32, device=device)
+    residual = torch.empty(n, device=device)
+    fitness = torch.empty(n, device=device)
+    if n == 0:
+        return out, status, residual, fitness
+    ws, ms, box_pixels = masked_scene(depth, K, det_frame, masks, rle, upm)
+    di = torch.as_tensor(det_idx, dtype=torch.int32).to(device)
+    chunk = max(1, min(n, WORKSPACE_BYTES // (box_pixels * 12 + 52 * H * W)))
+    for s in range(0, n, chunk):
+        sl = slice(s, min(n, s + chunk))
+        rendered, boxes = render_hypotheses(meshes_dev, labels[sl], poses[sl], K, frame_idx[sl], H, W, upm)
+        o = refine_rendered_masked(ms, ws, box_pixels, depth, K, di[sl].contiguous(), rendered, boxes, poses[sl],
+                                   **params)
+        out[sl], status[sl], residual[sl], fitness[sl] = o
+    return out, status, residual, fitness

@@ -444,6 +444,42 @@ int gp_icp_refine(int n_frames, int n_hyp, int height, int width, const int32_t*
                   const float* rendered_depth, const int64_t* boxes, const float* T0, const float* K,
                   const gp_icp_params_t* params, float* out_poses, int32_t* out_status, float* out_residual,
                   float* out_fitness, void* workspace, void* stream);
+/* Row f11, masked normals (opt-in; header comment of depth_icp.cu, steps 1' and 2'): the target map of each detection
+ * is smoothed within its own mask and stored over the mask's box only.  The detections are described on the HOST: */
+typedef struct gp_icp_mask_set {
+  int32_t n_det;                 /* 0 .. 65535 */
+  const int32_t* frame;          /* [n_det] frame of each detection, in [0, n_frames) */
+  const int32_t* boxes;          /* [n_det,4] mask boxes x0, y0, x1, y1, exclusive max, 0 <= x0 <= x1 <= W and
+                                    0 <= y0 <= y1 <= H (x0 == x1 or y0 == y1: an empty mask); the mask reads as 0
+                                    outside its box */
+  const int64_t* run_offsets;    /* [n_det+1] run-length masks: detection d owns counts[run_offsets[d] ..
+                                    run_offsets[d+1]), non-decreasing from >= 0; NULL for dense masks */
+} gp_icp_mask_set_t;
+/* Scene workspace bytes of the mask set, and box_pixels = the largest box area (the refine workspace holds
+ * n_hyp * box_pixels * 12 bytes).  tiles_offset / map_offset (nullable): byte offsets in the scene workspace of the
+ * mask tiles, u8, and of the maps, f32 x 6 per pixel; both hold the detections' boxes in order, each row-major
+ * (box h x box w), so detection d starts at the sum of the areas of the boxes before it. */
+int gp_icp_masked_query_sizes(int n_frames, int height, int width, const gp_icp_mask_set_t* set,
+                              size_t* workspace_bytes, int64_t* box_pixels, size_t* tiles_offset, size_t* map_offset);
+/* Writes the detection table to the start of the scene workspace and decodes every mask into a u8 box tile, from
+ * either masks u8 [n_det,H,W] (dense, nonzero = in the mask) or, with set->run_offsets, counts i32 (device) in the
+ * layout of gp_crop_resize_pad_rle (column-major runs, the first counting zeros; anything past the last run is 0).
+ * Two launches, plus one run scan per 256 detections for run-length masks. */
+int gp_icp_masked_decode(int n_frames, int height, int width, const gp_icp_mask_set_t* set, const uint8_t* masks,
+                         const int32_t* counts, void* workspace, void* stream);
+/* After gp_icp_masked_decode on the same workspace and mask set: depth f32 [n_frames,H,W], K f32 [n_frames,3,3].
+ * Writes each detection's map, f32 [box h, box w, 6] = (x, y, z, normal) with normals of the depth smoothed within its
+ * mask, in box order after the tiles.  Three launches. */
+int gp_icp_prepare_masked_scene(int n_frames, int height, int width, const gp_icp_mask_set_t* set, const float* depth,
+                                const float* K, float unit_per_m, void* workspace, void* stream);
+/* gp_icp_refine with hypothesis i refined against the map and mask of detection det_idx[i] (i32 [n_hyp], device; out
+ * of range: GP_ICP_INVALID); K is the scene's, the other arguments and outputs are gp_icp_refine's.  scene_workspace
+ * is the prepared scene; workspace holds n_hyp * box_pixels * 12 bytes of scratch. */
+int gp_icp_refine_masked(int n_frames, int height, int width, const gp_icp_mask_set_t* set, int n_hyp,
+                         const int32_t* det_idx, const float* rendered_depth, const int64_t* boxes, const float* T0,
+                         const float* K, const gp_icp_params_t* params, float* out_poses, int32_t* out_status,
+                         float* out_residual, float* out_fitness, const void* scene_workspace, void* workspace,
+                         void* stream);
 /* test hook: the exact median select of gp_icp_refine alone, in one 256-thread CTA.  bits u32 [n] (float bits of
  * non-negative distances; 0x7f800000 = no pair, skipped) -> out u32 [2]: m = the entries that are not 0x7f800000, and
  * the bits of the element of rank `rank` (0-based, ascending) among them, or 0x7f800000 when rank >= m.  n >= 1,

@@ -280,7 +280,7 @@ class GigaPose(LightningModule):
 
     @torch.no_grad()
     def refine_depth(self, dataset_name, predictions, depth, frame_idx=None, masks=None, hypotheses=1, *, K=None,
-                     rank=False, **params):
+                     rank=False, mask_normals=False, **params):
         """MegaPose's ICPRefiner.refine_poses on the output of `retrieve()`: the first `hypotheses` of the k poses of every
         detection are rendered and refined against the measured depth (gigapose_b200.icp.refine_icp).
 
@@ -295,8 +295,13 @@ class GigaPose(LightningModule):
         where not) are also scored against the depth (gigapose_b200.icp.score_hypotheses, row f10) and the collection
         carries `depth_counts` [B,hypotheses,4] (consistent, behind, front, missing pixels), `depth_score`
         [B,hypotheses] and `best_hypothesis` [B] (int64: the highest score, the lowest index on a tie); the order of the
-        hypotheses still does not change."""
-        from gigapose_b200.icp import DEFAULTS, refine_icp, score_hypotheses
+        hypotheses still does not change.
+
+        With `mask_normals=True` (row f11, an extension: the reference smooths the whole frame) `masks` is required, one
+        per detection, not per hypothesis: dense [B,H,W] or dict(counts=, offsets=) of COCO run-length masks
+        (offsets [B+1], bop_run's layout); every hypothesis is refined against target normals smoothed within its
+        detection's mask (gigapose_b200.icp.refine_icp_masked)."""
+        from gigapose_b200.icp import DEFAULTS, refine_icp, refine_icp_masked, score_hypotheses
         if K is None:
             raise TypeError("refine_depth needs K=, the frames' full-image intrinsics [F,3,3] or [3,3]")
         meshes = self.meshes[dataset_name]
@@ -314,10 +319,18 @@ class GigaPose(LightningModule):
                 raise ValueError("frame_idx is needed when depth holds several frames")
         frame_idx = np.asarray(torch.as_tensor(frame_idx).cpu()).reshape(-1)
         labels = object_indices(predictions.infos, len(meshes))
-        if masks is not None:
-            masks = torch.as_tensor(masks).to(poses.device).repeat_interleave(h, 0)
-        out, status, residual, fitness = refine_icp(meshes, np.repeat(labels, h), poses[:, :h].reshape(-1, 4, 4),
-                                                    depth, K, np.repeat(frame_idx, h), masks, **params)
+        if mask_normals:
+            if masks is None:
+                raise ValueError("mask_normals=True needs masks, dense [B,H,W] or dict(counts=, offsets=)")
+            dense, rle = (None, (masks["counts"], masks["offsets"])) if isinstance(masks, dict) else (masks, None)
+            out, status, residual, fitness = refine_icp_masked(
+                meshes, np.repeat(labels, h), poses[:, :h].reshape(-1, 4, 4), depth, K, frame_idx,
+                np.repeat(np.arange(B), h), dense, rle, **params)
+        else:
+            if masks is not None:
+                masks = torch.as_tensor(masks).to(poses.device).repeat_interleave(h, 0)
+            out, status, residual, fitness = refine_icp(meshes, np.repeat(labels, h), poses[:, :h].reshape(-1, 4, 4),
+                                                        depth, K, np.repeat(frame_idx, h), masks, **params)
         refined = predictions.clone()
         refined.register_tensor("poses_input", poses.clone())
         new = poses.clone()
