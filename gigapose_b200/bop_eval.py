@@ -8,10 +8,14 @@ contract), and the matching into recalls runs here in numpy.
 Row f8 scores the BOP 2024 6D-detection task (`evaluate_detection`): MSSD and MSPD of every kept estimate against every
 ground truth of its object in its image, then the greedy matching with ignored ground truths and the COCO average
 precision, all on the device (gp_bop_mssd_mspd, gp_bop_match, gp_bop_average_precision).  No depth images are read.
+
+Row f12 scores the BOP 2019 targets with ADD, ADD-S and the 2D-projection error (`evaluate_add`): the errors on the
+device (gp_bop_add), then minimum-error matching, the recalls at 0.1 d and 5 px and PoseCNN's AUC here in numpy.
 Usage:
 
     python -m gigapose_b200.bop_eval --results X.csv --dataset-dir D [--split test] [--out DIR]
     python -m gigapose_b200.bop_eval --task detection --results X.csv --dataset-dir D [--split test] [--out DIR]
+    python -m gigapose_b200.bop_eval --task add --results X.csv --dataset-dir D [--split test] [--out DIR]
 """
 from __future__ import annotations
 
@@ -41,7 +45,7 @@ MAX_SYM_DISC_STEP = 0.01        # continuous symmetries: the farthest vertex mov
 VISIB_GT_MIN = 0.1              # ground truths less visible than this are neither targets nor matchable
 Z_NEAR = 10.0                   # renders: near plane, model unit
 WORKSPACE_BYTES = 1 << 30       # device memory per chunk of images: measured depth, renders and the render keys
-MAX_PAIRS_PER_CALL = 1 << 18    # pairs per gp_bop_mssd_mspd call: ~140 B of poses, indices and errors each, ~37 MB
+MAX_PAIRS_PER_CALL = 1 << 18    # pairs per gp_bop_mssd_mspd / gp_bop_add call: ~140 B of poses, indices and errors each
 
 
 class BopEvalError(ValueError):
@@ -691,17 +695,212 @@ def evaluate_detection(results, dataset_dir, split="test", out_dir=None, device=
     return out
 
 
+# ---------------------------------------------------------------------------------------------------- ADD, ADD-S, proj
+# Row f12: the metrics of the LM / LM-O (ADD(-S) recall at 0.1 d), YCB-V (AUC of ADD-S and ADD(-S) up to 10 cm) and
+# 2D-projection (5 px) tables, on the BOP 2019 targets of `prepare`.  The per-pair errors are gp_bop_add's (definitions
+# in csrc/bop_eval.cu, above add_kernel); the matching, recalls and AUCs run here on the host.  This is this
+# repository's restatement of MegaPose's vendored pieces (dists_add / dists_add_symmetric, get_top_n_ids, add_valid_gt,
+# match_poses, compute_auc_posecnn); the meter that combined them is not part of the reference.
+ADD_THRESHOLD = 0.1             # x diameter, ADD-S and ADD(-S)
+PROJ_THRESHOLD = 5.0            # px, unscaled
+AUC_MAX_M = 0.1                 # PoseCNN's AUC cap, metres
+ADD_METRICS = ("add(-s)", "add-s", "proj")
+
+
+def is_symmetric(info):
+    """An object that declares a discrete or a continuous symmetry in models_info.json: ADD(-S) takes its ADD-S."""
+    return bool(info.get("symmetries_discrete")) or bool(info.get("symmetries_continuous"))
+
+
+def add_errors(obj_idx, vertex_offsets, vertices, K, frame_idx, pose_est, pose_gt):
+    """gp_bop_add on device tensors (offsets are host int sequences), at most MAX_PAIRS_PER_CALL pairs per call and no
+    call for no pairs -> f64 [n, 3] = (ADD, ADD-S, proj)."""
+    n = obj_idx.shape[0]
+    out = torch.empty(n, 3, dtype=torch.float64, device=vertices.device)
+    if n == 0:
+        return out
+    vo = (C.c_int32 * len(vertex_offsets))(*vertex_offsets)
+    max_v = max(b - a for a, b in zip(vertex_offsets[:-1], vertex_offsets[1:]))
+    n_chunks = -(-max_v // _lib.BOP_ADD_CHUNK)
+    ws = torch.empty(min(n, MAX_PAIRS_PER_CALL) * n_chunks * 3, dtype=torch.float64, device=vertices.device)
+    lib, stream = _lib.load(), torch.cuda.current_stream(vertices.device).cuda_stream
+    rows = [(t.data_ptr(), t.stride(0) * t.element_size()) for t in (obj_idx, frame_idx, pose_est, pose_gt, out)]
+    for p0 in range(0, n, MAX_PAIRS_PER_CALL):
+        o, f, pe, pg, d = (ptr + p0 * step for ptr, step in rows)
+        check(lib.gp_bop_add(min(MAX_PAIRS_PER_CALL, n - p0), len(vertex_offsets) - 1, o, vo, vertices.data_ptr(),
+                             K.shape[0], K.data_ptr(), f, pe, pg, ws.data_ptr(), d, stream))
+    return out
+
+
+def compute_add_errors(setup, device="cuda", stage_ms=None):
+    """ADD, ADD-S and proj of every (kept estimate, ground truth of its object) pair of the targets of `prepare`, on
+    the device.  -> dict of numpy arrays over the pairs (the layout of `_pair_rows`): group (target index), est (result
+    index), gt (instance index in scene_gt), add, adds, proj (f64, model unit and px).  `stage_ms` (a dict) receives
+    the CUDA-event milliseconds of the stage `add`."""
+    device = _lib.cuda_device(device, "BOP evaluation")
+    results, groups, scenes = setup["results"], setup["groups"], setup["scenes"]
+    pairs = _pair_rows(groups, range(len(groups)), setup["images"])
+    n = len(pairs["group"])
+    out = dict(pairs, add=np.zeros(0), adds=np.zeros(0), proj=np.zeros(0))
+    del out["frame"]
+    if n == 0:
+        return out
+    obj_ids = sorted({groups[gi]["obj_id"] for gi in set(pairs["group"].tolist())})
+    if len(obj_ids) > _lib.BOP_MAX_OBJECTS:
+        raise BopEvalError(f"at most {_lib.BOP_MAX_OBJECTS} objects per evaluation")
+    oidx = {o: i for i, o in enumerate(obj_ids)}
+    stages = _Stages(stage_ms is not None)
+    with torch.cuda.device(device):
+        _, vertices, _, vo, _ = _object_tables(setup, obj_ids, device)
+        K = torch.as_tensor(np.stack([scenes[s]["K"][im] for s, im in setup["images"]]), dtype=torch.float32,
+                            device=device).contiguous()
+        gl, el, kl = pairs["group"].tolist(), pairs["est"].tolist(), pairs["gt"].tolist()
+        pose_est = np.stack([_pose(results[e]["R"], results[e]["t"]) for e in el]).astype(np.float32)
+        gts = [scenes[groups[gi]["scene_id"]]["gt"][groups[gi]["im_id"]][k] for gi, k in zip(gl, kl)]
+        pose_gt = np.stack([_pose(g["R"], g["t"]) for g in gts]).astype(np.float32)
+        t = lambda a: torch.as_tensor(np.ascontiguousarray(a), device=device)
+        obj_d = t(np.array([oidx[groups[gi]["obj_id"]] for gi in gl], np.int32))
+        frame_d = t(pairs["frame"].astype(np.int32))
+        with stages("add"):
+            err = add_errors(obj_d, vo, vertices, K, frame_d, t(pose_est), t(pose_gt))
+        err = err.cpu().numpy()
+    if stage_ms is not None:
+        stage_ms.update(stages.totals())
+    out.update(add=err[:, 0].copy(), adds=err[:, 1].copy(), proj=err[:, 2].copy())
+    return out
+
+
+def match_min_error(err, valid):
+    """Minimum-error matching of one target (MegaPose's match_poses rule): err [n_est, n_gt] with the estimates in
+    descending score order, valid [n_gt].  Each estimate in turn takes the unmatched valid ground truth with the
+    smallest error (strict `<` against a running best that starts at +inf, so the lowest index wins a tie and an inf or
+    NaN error never matches); there is no threshold.  -> (matched error per ground truth [n_gt], inf when unmatched;
+    the matching estimate's row [n_gt], -1 when unmatched)."""
+    err = np.asarray(err, np.float64).reshape(-1, len(valid))
+    out = np.full(len(valid), np.inf)
+    row_of = np.full(len(valid), -1, np.int64)
+    for a, row in enumerate(err):
+        best, best_j = np.inf, -1
+        for j in range(len(valid)):
+            if valid[j] and row_of[j] < 0 and row[j] < best:
+                best, best_j = row[j], j
+        if best_j >= 0:
+            row_of[best_j] = a
+            out[best_j] = best
+    return out, row_of
+
+
+def auc_posecnn(errors_m):
+    """PoseCNN's area under the accuracy-threshold curve, as MegaPose's compute_auc_posecnn computes it: the errors
+    (metres, inf for a missed target) sorted; accuracy (k + 1) / n at the k-th; errors above AUC_MAX_M (and inf or NaN)
+    dropped, so an error of exactly AUC_MAX_M counts; the precision envelope made non-decreasing; the step area over
+    the recall points [0, kept errors..., AUC_MAX_M], times 10 (= 1 / AUC_MAX_M, applied as a multiplication the way
+    MegaPose does).  NaN when no error is within AUC_MAX_M."""
+    d = np.sort(np.asarray(errors_m, np.float64))
+    acc = np.cumsum(np.ones(len(d))) / len(d)
+    keep = d <= AUC_MAX_M
+    if not keep.any():
+        return float("nan")
+    rec = np.concatenate(([0.0], d[keep], [AUC_MAX_M]))
+    pre = np.maximum.accumulate(np.concatenate(([0.0], acc[keep], [acc[keep][-1]])))
+    i = np.nonzero(rec[1:] != rec[:-1])[0] + 1
+    return float(((rec[i] - rec[i - 1]) * pre[i]).sum() * 10.0)
+
+
+def add_scores(setup, errors):
+    """Host half of `evaluate_add`: per target, each metric matched on its own error (`match_min_error`), then the
+    recalls (matched valid ground truths with error < threshold over n_targets; 0.1 x diameter for ADD-S and ADD(-S),
+    5 px for proj) and the AUCs of ADD-S and ADD(-S) (`auc_posecnn` on mm / 1000, inf for an unmatched target), over
+    all targets and per object.  The targets are the valid ground truths, target group after target group.
+    -> dict(n_targets, matched {metric: matched error f64 [n_targets], inf if missed}, matched_est {metric: result
+    index of the matching estimate [n_targets], -1 if missed}, target_obj [n_targets], target_gt [(target group,
+    instance index)], recall {metric}, auc {metric}, objects {obj_id: dict(n_targets, recall, auc)})."""
+    groups, info = setup["groups"], setup["info"]
+    pos = [({e: i for i, e in enumerate(g["est"])}, {k: i for i, k in enumerate(g["gt"])}) for g in groups]
+    tables = [{m: np.full((len(g["est"]), len(g["gt"])), np.inf) for m in ADD_METRICS} for g in groups]
+    for p in range(len(errors["group"])):
+        gi = int(errors["group"][p])
+        a, b = pos[gi][0][int(errors["est"][p])], pos[gi][1][int(errors["gt"][p])]
+        sym = is_symmetric(info[groups[gi]["obj_id"]])
+        tables[gi]["add(-s)"][a, b] = errors["adds"][p] if sym else errors["add"][p]
+        tables[gi]["add-s"][a, b] = errors["adds"][p]
+        tables[gi]["proj"][a, b] = errors["proj"][p]
+    matched, matched_est = {m: [] for m in ADD_METRICS}, {m: [] for m in ADD_METRICS}
+    target_obj, target_gt, thr = [], [], {m: [] for m in ADD_METRICS}
+    for gi, (g, tab) in enumerate(zip(groups, tables)):
+        v = np.asarray(g["valid"], bool)
+        for m in ADD_METRICS:
+            e, a = match_min_error(tab[m], v)
+            matched[m].append(e[v])
+            matched_est[m].append(np.array([g["est"][i] if i >= 0 else -1 for i in a[v]], np.int64))
+        target_gt += [(gi, k) for k, ok in zip(g["gt"], v) if ok]
+        n = int(v.sum())
+        target_obj += [g["obj_id"]] * n
+        d = info[g["obj_id"]]["diameter"]
+        thr["add(-s)"] += [ADD_THRESHOLD * d] * n
+        thr["add-s"] += [ADD_THRESHOLD * d] * n
+        thr["proj"] += [PROJ_THRESHOLD] * n
+    matched = {m: np.concatenate(v) if v else np.zeros(0) for m, v in matched.items()}
+    matched_est = {m: np.concatenate(v) if v else np.zeros(0, np.int64) for m, v in matched_est.items()}
+    target_obj = np.asarray(target_obj, np.int64)
+    thr = {m: np.asarray(v, np.float64) for m, v in thr.items()}
+
+    def scores(sel):
+        n = int(sel.sum())
+        rec = {m: float(np.count_nonzero(matched[m][sel] < thr[m][sel]) / max(n, 1)) for m in ADD_METRICS}
+        auc = {m: auc_posecnn(matched[m][sel] / 1000.0) if n else float("nan") for m in ("add(-s)", "add-s")}
+        return n, rec, auc
+
+    n_targets, recall, auc = scores(np.ones(len(target_obj), bool))
+    objects = {}
+    for o in sorted(set(target_obj.tolist())):
+        n, rec, a = scores(target_obj == o)
+        objects[o] = dict(n_targets=n, recall=rec, auc=a)
+    return dict(n_targets=n_targets, matched=matched, matched_est=matched_est, target_obj=target_obj,
+                target_gt=target_gt, recall=recall, auc=auc, objects=objects)
+
+
+def _add_json(n_targets, recall, auc):
+    return {"add(-s)_0.1d": recall["add(-s)"], "add-s_0.1d": recall["add-s"], "proj_5px": recall["proj"],
+            "auc_add(-s)": auc["add(-s)"], "auc_add-s": auc["add-s"], "n_targets": n_targets}
+
+
+@torch.no_grad()
+def evaluate_add(results, dataset_dir, split="test", out_dir=None, device="cuda",
+                 targets_name="test_targets_bop19.json", stage_ms=None):
+    """ADD, ADD-S and 2D-projection scores of `results` (a csv path or a list of `load_bop_results` dicts) on the BOP
+    2019 targets of a dataset directory; needs no depth images.  -> dict(errors (per pair: group, est, gt, add, adds,
+    proj), matched / matched_est / target_obj / target_gt (per target, see `add_scores`), recall / auc {metric}, n_targets,
+    objects {obj_id: dict(n_targets, recall, auc)}, scores (the JSON below)).  Metrics: "add(-s)" (ADD-S for an object
+    with declared symmetries, else ADD), "add-s", "proj".  With `out_dir`, writes out_dir/scores_add.json:
+    add(-s)_0.1d, add-s_0.1d, proj_5px (recalls), auc_add(-s), auc_add-s (NaN when no target is within 0.1 m),
+    n_targets, and the same keys per object under "objects" {obj_id}.  `stage_ms` (a dict) receives the CUDA-event
+    milliseconds of the stage `add`."""
+    setup = prepare(results, dataset_dir, split, targets_name)
+    errors = compute_add_errors(setup, device, stage_ms=stage_ms)
+    s = add_scores(setup, errors)
+    scores = dict(_add_json(s["n_targets"], s["recall"], s["auc"]),
+                  objects={str(o): _add_json(v["n_targets"], v["recall"], v["auc"]) for o, v in s["objects"].items()})
+    _write_scores(out_dir, "scores_add.json", scores)
+    return dict(s, errors=errors, scores=scores)
+
+
 def main(argv=None):
     ap = argparse.ArgumentParser(description="BOP pose-error evaluation on the GPU: the BOP 2019 localization task "
-                                             "(VSD, MSSD, MSPD, AR) or the BOP 2024 6D-detection task (MSSD, MSPD, mAP)")
+                                             "(VSD, MSSD, MSPD, AR), the BOP 2024 6D-detection task (MSSD, MSPD, mAP) "
+                                             "or ADD / ADD-S / 2D-projection scores on the BOP 2019 targets")
     ap.add_argument("--results", required=True, help="BOP results csv")
     ap.add_argument("--dataset-dir", required=True)
     ap.add_argument("--split", default="test")
-    ap.add_argument("--task", choices=("localization", "detection"), default="localization")
-    ap.add_argument("--out", default=None, help="directory for scores_bop19.json / scores_bop24.json (default: next to "
-                                                "the csv)")
+    ap.add_argument("--task", choices=("localization", "detection", "add"), default="localization")
+    ap.add_argument("--out", default=None, help="directory for scores_bop19.json / scores_bop24.json / scores_add.json "
+                                                "(default: next to the csv)")
     a = ap.parse_args(argv)
     out_dir = a.out if a.out is not None else os.path.dirname(os.path.abspath(a.results))
+    if a.task == "add":
+        res = evaluate_add(a.results, a.dataset_dir, a.split, out_dir=out_dir)
+        print(json.dumps({k: v for k, v in res["scores"].items() if k != "objects"}))
+        return
     if a.task == "detection":
         res = evaluate_detection(a.results, a.dataset_dir, a.split, out_dir=out_dir)
         print(json.dumps({k: res[k] for k in ("map", "map_mssd", "map_mspd", "objects", "average_time_per_image")}))

@@ -50,6 +50,8 @@
 //  suffix max over the slots gives q_k = max over slots c > k.  AP = (((q_0 + q_1) + q_2) + ... + q_{K-1}) / K in fp64,
 //  summed on one thread.  Every step is an integer operation, an exact max or one rounded fp64 operation, so
 //  oracle/bop24_port.py (detection_labels, average_precision) restates it bit for bit.
+//
+// Row f12: ADD, ADD-S and the 2D-projection error (gp_bop_add); the definitions are the comment above add_kernel.
 #include "../../include/gigapose_b200.h"
 #include "gigapose_kernels.h"
 
@@ -366,6 +368,128 @@ ap_kernel(int n_theta, int n_est, const int8_t* __restrict__ labels, const int32
   }
 }
 
+// ---------------------------------------------------------------------------------------------------- row f12
+// ADD (Hinterstoisser et al., ACCV 2012), ADD-S (the same paper's measure for indistinguishable views; PoseCNN's "ADD-S")
+// and the 2D-projection error (Brachmann et al., CVPR 2016) of (estimate, ground truth) pairs of the same object.  P =
+// [R | t] object -> camera; the model points x are all vertices of the object (N of them), in the model unit.
+//   ADD   = mean over x of |P_est x - P_gt x|
+//   ADD-S = mean over the ground-truth points g_j = P_gt x_j of min over i of |g_j - P_est x_i|   (the nearest
+//           estimated point of each ground-truth point: the direction of MegaPose's dists_add_symmetric and of the BOP
+//           toolkit's adi)
+//   proj  = mean over x of the pixel distance between the projections of P_est x and P_gt x with the frame's K
+// Per-vertex arithmetic is mssd_mspd_kernel's with S = I: e = P_est x and g = P_gt x by `affine`, each row
+// ((A0 x + A1 y) + A2 z) + A3; squared distance `sq3` = (dx dx + dy dy) + dz dz with d = e - g; projection `project`,
+// u = (K00 x + K01 y) / z + K02, v = (K11 y) / z + K12, squared pixel distance du du + dv dv; every operation one fp32
+// rounding, no FMA contraction.  The per-point distances are one __fsqrt_rn of the squared term; for ADD-S the min over
+// i is taken on the squared terms first (as unsigned bits: every term is >= 0 or NaN, so it is the float order with NaN
+// above +inf; a NaN term wins only when every term is NaN), then one sqrt.  The min is exact, so the schedule does not
+// matter.
+// Sums: vertex j belongs to chunk c = j / GP_BOP_ADD_CHUNK.  Each chunk's partial is the fp64 sum of its per-point
+// distances widened to fp64, left to right in vertex order, starting from the first; the finishing launch adds the
+// partials left to right in chunk order and divides once by (double)N (__ddiv_rn).  Nothing else enters the order, so
+// oracle/add_port.py restates it bit for bit.  A pair whose object or frame index is out of range gets NaN; a NaN pose
+// gives NaN.
+// Schedule: grid (pair, chunk), kThreads threads, thread t holding the ground-truth vertices c * CHUNK + t + kThreads r
+// (r < kAddPerThread) in registers with their ADD and proj terms; the estimated points of the object are transformed into
+// shared-memory tiles of kAddTile points and streamed past them.  The partials go to the workspace
+// (f64 [n_pairs, n_chunks, 3]); add_finish_kernel sums them, one thread per (pair, metric).
+constexpr int kAddPerThread = GP_BOP_ADD_CHUNK / kThreads;
+constexpr int kAddTile = 1024;
+static_assert(kAddPerThread * kThreads == GP_BOP_ADD_CHUNK, "chunk = threads x vertices per thread");
+
+struct VertexTable {                  // host offsets, by value: object o owns vertices [off[o], off[o + 1])
+  int32_t off[GP_BOP_MAX_OBJECTS + 1];
+};
+
+__global__ void __launch_bounds__(kThreads, 2)
+add_kernel(int n_objects, const int32_t* __restrict__ obj_idx, VertexTable tab, const float* __restrict__ vertices,
+           int n_frames, const float* __restrict__ Kmat, const int32_t* __restrict__ frame_idx,
+           const float* __restrict__ pose_est, const float* __restrict__ pose_gt, double* __restrict__ partial) {
+  __shared__ float4 sE[kAddTile];
+  __shared__ float sDist[3][GP_BOP_ADD_CHUNK];
+  __shared__ float sPe[16], sPg[16], sK[9];
+  const int pair = blockIdx.x, chunk = blockIdx.y, tid = threadIdx.x;
+  const int o = obj_idx[pair], f = frame_idx[pair];
+  if (o < 0 || o >= n_objects || f < 0 || f >= n_frames) return;   // add_finish_kernel writes NaN
+  const int v0 = tab.off[o], n = tab.off[o + 1] - v0;
+  const int j0 = chunk * GP_BOP_ADD_CHUNK;
+  if (j0 >= n) return;
+  if (tid < 16) { sPe[tid] = pose_est[16 * (size_t)pair + tid]; sPg[tid] = pose_gt[16 * (size_t)pair + tid]; }
+  if (tid < 9) sK[tid] = Kmat[9 * (size_t)f + tid];
+  __syncthreads();
+  float g[kAddPerThread][3];
+  unsigned best[kAddPerThread];
+#pragma unroll
+  for (int r = 0; r < kAddPerThread; ++r) {
+    const int j = j0 + tid + kThreads * r;
+    best[r] = 0xffffffffu;
+    if (j < n) {
+      const float* p = vertices + 3 * (size_t)(v0 + j);
+      const float x = p[0], y = p[1], z = p[2];
+      float e[3], ue, ve, ug, vg;
+      affine(sPe, x, y, z, e);
+      affine(sPg, x, y, z, g[r]);
+      project(sK, e, ue, ve);
+      project(sK, g[r], ug, vg);
+      const float du = __fsub_rn(ue, ug), dv = __fsub_rn(ve, vg);
+      sDist[0][tid + kThreads * r] =
+          __fsqrt_rn(sq3(__fsub_rn(e[0], g[r][0]), __fsub_rn(e[1], g[r][1]), __fsub_rn(e[2], g[r][2])));
+      sDist[2][tid + kThreads * r] = __fsqrt_rn(__fadd_rn(__fmul_rn(du, du), __fmul_rn(dv, dv)));
+    } else {
+      g[r][0] = g[r][1] = g[r][2] = 0.f;
+    }
+  }
+  for (int base = 0; base < n; base += kAddTile) {
+    const int m = min(kAddTile, n - base);
+    __syncthreads();                                         // the previous tile has been read
+    for (int i = tid; i < m; i += kThreads) {
+      const float* p = vertices + 3 * (size_t)(v0 + base + i);
+      float e[3];
+      affine(sPe, p[0], p[1], p[2], e);
+      sE[i] = make_float4(e[0], e[1], e[2], 0.f);
+    }
+    __syncthreads();
+#pragma unroll 4
+    for (int i = 0; i < m; ++i) {
+      const float4 e = sE[i];                                // the same address on every lane: a broadcast
+#pragma unroll
+      for (int r = 0; r < kAddPerThread; ++r)
+        best[r] = min(best[r], __float_as_uint(sq3(__fsub_rn(e.x, g[r][0]), __fsub_rn(e.y, g[r][1]),
+                                                   __fsub_rn(e.z, g[r][2]))));
+    }
+  }
+#pragma unroll
+  for (int r = 0; r < kAddPerThread; ++r)
+    if (j0 + tid + kThreads * r < n) sDist[1][tid + kThreads * r] = __fsqrt_rn(__uint_as_float(best[r]));
+  __syncthreads();
+  if (tid < 3) {
+    const int cnt = min(GP_BOP_ADD_CHUNK, n - j0);
+    double s = (double)sDist[tid][0];
+    for (int j = 1; j < cnt; ++j) s = __dadd_rn(s, (double)sDist[tid][j]);
+    partial[((size_t)pair * gridDim.y + chunk) * 3 + tid] = s;
+  }
+}
+
+__global__ void __launch_bounds__(kThreads)
+add_finish_kernel(int n_pairs, int n_chunks, int n_objects, const int32_t* __restrict__ obj_idx, VertexTable tab,
+                  int n_frames, const int32_t* __restrict__ frame_idx, const double* __restrict__ partial,
+                  double* __restrict__ out) {
+  const long long t = (long long)blockIdx.x * kThreads + threadIdx.x;
+  if (t >= 3ll * n_pairs) return;
+  const int pair = (int)(t / 3), m = (int)(t % 3);
+  const int o = obj_idx[pair], f = frame_idx[pair];
+  if (o < 0 || o >= n_objects || f < 0 || f >= n_frames) {
+    out[t] = __longlong_as_double(0x7ff8000000000000ll);
+    return;
+  }
+  const int n = tab.off[o + 1] - tab.off[o];
+  const int nc = (n + GP_BOP_ADD_CHUNK - 1) / GP_BOP_ADD_CHUNK;
+  const double* p = partial + (size_t)pair * n_chunks * 3 + m;
+  double s = p[0];
+  for (int c = 1; c < nc; ++c) s = __dadd_rn(s, p[3 * c]);
+  out[t] = __ddiv_rn(s, (double)n);
+}
+
 }  // namespace
 
 extern "C" int gp_bop_vsd(int n_pairs, int n_frames, int height, int width, const float* depth_test, const float* K,
@@ -426,6 +550,38 @@ extern "C" int gp_bop_mssd_mspd(int n_pairs, int n_objects, const int32_t* obj_i
   GP_CUDA(gp::launch_ex(mssd_mspd_kernel, dim3(n_pairs, (max_syms + kSymPerCta - 1) / kSymPerCta), kThreads, 0, st, 1,
                         false, n_objects, obj_idx, tab, vertices, syms, n_frames, K, frame_idx, pose_est, pose_gt, mssd,
                         mspd));
+  return GP_OK;
+}
+
+extern "C" int gp_bop_add(int n_pairs, int n_objects, const int32_t* obj_idx, const int32_t* vertex_offsets,
+                          const float* vertices, int n_frames, const float* K, const int32_t* frame_idx,
+                          const float* pose_est, const float* pose_gt, void* workspace, double* out, void* stream) {
+  if (n_pairs < 1) return fail(GP_ERR_INVALID, "n_pairs %d must be >= 1", n_pairs);
+  if (n_objects < 1 || n_objects > GP_BOP_MAX_OBJECTS)
+    return fail(GP_ERR_INVALID, "n_objects %d outside [1, %d]", n_objects, GP_BOP_MAX_OBJECTS);
+  if (n_frames < 1) return fail(GP_ERR_INVALID, "n_frames %d must be >= 1", n_frames);
+  if (!vertex_offsets) return fail(GP_ERR_INVALID, "null offsets");
+  VertexTable tab;
+  int max_v = 0;
+  for (int o = 0; o <= n_objects; ++o) {
+    tab.off[o] = vertex_offsets[o];
+    if (o == 0 ? vertex_offsets[0] != 0 : vertex_offsets[o] <= vertex_offsets[o - 1])
+      return fail(GP_ERR_INVALID, "bad vertex offsets at object %d: they must start at 0 and increase strictly", o);
+    if (o > 0) max_v = max(max_v, vertex_offsets[o] - vertex_offsets[o - 1]);
+  }
+  for (int o = n_objects + 1; o <= GP_BOP_MAX_OBJECTS; ++o) tab.off[o] = 0;
+  const int n_chunks = (max_v + GP_BOP_ADD_CHUNK - 1) / GP_BOP_ADD_CHUNK;
+  if (n_chunks > 65535) return fail(GP_ERR_INVALID, "an object of %d vertices has more than 65535 chunks", max_v);
+  if (!obj_idx || !vertices || !K || !frame_idx || !pose_est || !pose_gt || !workspace || !out)
+    return fail(GP_ERR_INVALID, "null argument");
+  if (reinterpret_cast<uintptr_t>(workspace) % 8) return fail(GP_ERR_INVALID, "workspace must be 8-byte aligned");
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  double* partial = static_cast<double*>(workspace);
+  GP_CUDA(gp::launch_ex(add_kernel, dim3(n_pairs, n_chunks), kThreads, 0, st, 1, false, n_objects, obj_idx, tab,
+                        vertices, n_frames, K, frame_idx, pose_est, pose_gt, partial));
+  GP_CUDA(gp::launch_ex(add_finish_kernel, (unsigned)((3ll * n_pairs + kThreads - 1) / kThreads), kThreads, 0, st, 1,
+                        false, n_pairs, n_chunks, n_objects, obj_idx, tab, n_frames, frame_idx,
+                        static_cast<const double*>(partial), out));
   return GP_OK;
 }
 

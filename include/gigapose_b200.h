@@ -375,6 +375,22 @@ int gp_bop_average_precision(int n_objects, int n_theta, int n_est, const int8_t
                              const int32_t* rank, const int32_t* n_valid, int n_recall, const double* recall_thresholds,
                              double* ap, void* stream);
 
+/* --- row f12: ADD, ADD-S and the 2D-projection error (LM / LM-O's ADD(-S) recall at 0.1 d, YCB-V's AUC, the 5 px
+ * projection recall).  The definitions, with the fp32 / fp64 operation order, are the comment above add_kernel in
+ * gigapose_b200/csrc/bop_eval.cu.  Needs no handle. ------------------------------------------------------------------ */
+#define GP_BOP_ADD_CHUNK 1024          /* ground-truth vertices per partial sum of gp_bop_add */
+/* ADD, ADD-S (model unit) and proj (px) of n_pairs (estimate, ground truth) pairs over every vertex of the pair's object.
+ *   obj_idx i32 [n_pairs] (0-based), vertices f32 [sum V_o, 3] concatenated per object with HOST offsets
+ *   vertex_offsets i32 [n_objects + 1] (0 first, strictly increasing); K f32 [n_frames,3,3], frame_idx i32 [n_pairs],
+ *   pose_est / pose_gt f32 [n_pairs,4,4] object -> camera (gp_bop_mssd_mspd's tables without the symmetries);
+ *   workspace of 24 * n_pairs * ceil(max_o V_o / GP_BOP_ADD_CHUNK) bytes, 8-byte aligned (the per-chunk partial sums;
+ *   at most 65535 chunks).
+ * Output out f64 [n_pairs, 3] = (ADD, ADD-S, proj); a pair whose object or frame index is out of range gets NaN. Two
+ * launches, in stream order. */
+int gp_bop_add(int n_pairs, int n_objects, const int32_t* obj_idx, const int32_t* vertex_offsets, const float* vertices,
+               int n_frames, const float* K, const int32_t* frame_idx, const float* pose_est, const float* pose_gt,
+               void* workspace, double* out, void* stream);
+
 /* --- row f6: depth refinement of the coarse poses (MegaPose's ICPRefiner, src/megapose/inference/icp_refiner.py:134-287,
  * with a GPU point-to-plane ICP in place of OpenCV's ppf_match_3d_ICP).  The full contract is the header comment of
  * gigapose_b200/csrc/depth_icp.cu.  Needs no handle. ------------------------------------------------------------- */
