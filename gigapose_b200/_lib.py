@@ -101,6 +101,31 @@ class GpIcpMaskSet(C.Structure):
 ICP_OK, ICP_TOO_FEW_POINTS, ICP_DEGENERATE, ICP_RESIDUAL, ICP_INVALID, ICP_LOST = 0, 1, 2, 3, 4, 5
 
 
+class GpTeaserGnc(C.Structure):
+    """gp_teaser_gnc_t: one GNC-TLS iteration of one hypothesis (112 bytes; np.dtype(GpTeaserGnc) reads an array)."""
+    _fields_ = [("iteration", C.c_int32), ("members", C.c_int32), ("stopped", C.c_int32), ("reserved", C.c_int32),
+                ("mu", C.c_double), ("cost", C.c_double), ("max_residual", C.c_double), ("R", C.c_double * 9)]
+
+
+class GpTeaserDebug(C.Structure):
+    _fields_ = [("counts", C.c_void_p), ("points", C.c_void_p), ("samples", C.c_void_p), ("adjacency", C.c_void_p),
+                ("clique", C.c_void_p), ("gnc", C.c_void_p), ("gnc_weights", C.c_void_p),
+                ("gnc_capacity", C.c_int32), ("stop_after", C.c_int32), ("transform", C.c_void_p)]
+
+
+class GpTeaserParams(C.Structure):
+    _fields_ = [("unit_per_m", C.c_float), ("min_points", C.c_int32), ("n_points", C.c_int32),
+                ("noise_bound", C.c_float), ("cbar2", C.c_float), ("min_inliers", C.c_int32),
+                ("gnc_factor", C.c_float), ("gnc_max_iters", C.c_int32), ("gnc_cost_threshold", C.c_double),
+                ("clique_budget", C.c_int64), ("debug", GpTeaserDebug)]
+
+
+# gp_teaser_refine statuses (GP_TEASER_*)
+TEASER_OK, TEASER_TOO_FEW_POINTS, TEASER_CLIQUE_TOO_SMALL, TEASER_CLIQUE_BUDGET = 0, 1, 2, 3
+TEASER_TOO_FEW_INLIERS, TEASER_INVALID = 4, 5
+TEASER_MAX_POINTS = 1024       # GP_TEASER_MAX_POINTS
+
+
 # every symbol include/gigapose_b200.h declares: name -> (restype, argtypes)
 SYMBOLS = {
     "gp_last_error": (C.c_char_p, []),
@@ -183,6 +208,10 @@ SYMBOLS = {
     "gp_debug_icp_select": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
     "gp_depth_score": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
                                  C.c_void_p, C.c_float, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "gp_teaser_query_sizes": (C.c_int, [C.c_int, C.c_int, C.c_int, C.POINTER(C.c_size_t)]),
+    "gp_teaser_refine": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                   C.c_void_p, C.c_void_p, C.POINTER(GpTeaserParams), C.c_void_p, C.c_void_p,
+                                   C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "gp_ist_trunk_query_sizes":(C.c_int, [C.c_int, C.POINTER(C.c_size_t), C.POINTER(C.c_size_t)]),
     "gp_ist_trunk_create": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                       C.POINTER(C.c_void_p)]),

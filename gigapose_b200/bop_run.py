@@ -17,11 +17,15 @@ run_depth_refiner passes none, pose_estimator.py:501-503), the refined hypothese
 
 Row f11, `--refine-masks` with `--refine-depth H`: each kept instance is refined with its own CNOS mask, the run-length
 encoding decoded on the GPU over the mask's box, as the target set and as the region its target normals are smoothed
-in (`GigaPose.refine_depth(mask_normals=True)`); the csv is `..._{run_id}_icp_masked.csv`.  Usage:
+in (`GigaPose.refine_depth(mask_normals=True)`); the csv is `..._{run_id}_icp_masked.csv`.
+
+Row f13, `--depth-refiner teaserpp` with `--refine-depth H`: the hypotheses go through MegaPose's TEASER++ refiner
+(`GigaPose.refine_depth(refiner="teaserpp")`) instead of the ICP, with the same ranking; the csv is
+`..._{run_id}_teaserpp.csv`.  Usage:
 
     python -m gigapose_b200.bop_run --dataset-dir D --checkpoint gigaPose_v1.ckpt --template-poses P.npy
-        [--setting localization|detection] [--detections FILE] [--out DIR] [--refine-depth H [--refine-masks]]
-        [--evaluate]
+        [--setting localization|detection] [--detections FILE] [--out DIR]
+        [--refine-depth H [--refine-masks | --depth-refiner teaserpp]] [--evaluate]
 """
 from __future__ import annotations
 
@@ -433,7 +437,7 @@ def select_rle(rle, selected):
 
 
 @torch.no_grad()
-def refine_image(model, p, i, kept, depth, hypotheses, out_dir, masks=None):
+def refine_image(model, p, i, kept, depth, hypotheses, out_dir, masks=None, refiner="icp"):
     """Row f10 for image i of the plan: the first `hypotheses` poses of each of the `kept` instances (the collection
     `eval_retrieval` returns after its filter, with `time` and `detection_time`) go through
     `GigaPose.refine_depth(rank=True)` against `depth` (f32 [H,W] in the model unit, host or device), and
@@ -442,7 +446,8 @@ def refine_image(model, p, i, kept, depth, hypotheses, out_dir, masks=None):
     measured with CUDA events from the depth upload to the end of the scoring, plus `hypothesis` (the index chosen) and
     its `icp_status`, which the csv writer does not read.  With `masks` = (counts, offsets), the run-length masks of
     the kept instances in their order, they refine with `mask_normals=True`; `refinement_time` then covers the mask
-    decode.  -> the refined collection."""
+    decode.  With `refiner="teaserpp"` the hypotheses go through the TEASER++ refiner (row f13) and the npz holds
+    `teaser_status` in place of `icp_status`.  -> the refined collection."""
     s, im = p["images"][i]
     device = kept.pred_poses.device
     n = len(kept)
@@ -451,12 +456,15 @@ def refine_image(model, p, i, kept, depth, hypotheses, out_dir, masks=None):
     depth = torch.as_tensor(depth).to(device, non_blocking=True)
     K = torch.as_tensor(p["cameras"][s][im], dtype=torch.float64).float()
     extra = {} if masks is None else dict(masks=dict(counts=masks[0], offsets=masks[1]), mask_normals=True)
+    if refiner != "icp":
+        extra["refiner"] = refiner
     refined = model.refine_depth(p["name"], kept, depth[None], frame_idx=np.zeros(n, np.int64), hypotheses=hypotheses,
                                  K=K, rank=True, **extra)
     rows = torch.arange(n, device=device)
     poses = refined.pred_poses[rows, refined.best_hypothesis]
     scores = kept.scores[rows, refined.best_hypothesis]
-    status = refined.icp_status[rows, refined.best_hypothesis]
+    status_key = "icp_status" if refiner == "icp" else "teaser_status"
+    status = getattr(refined, status_key)[rows, refined.best_hypothesis]
     stop.record()
     stop.synchronize()
     labels = np.asarray(kept.infos.label).astype(np.int32)
@@ -469,26 +477,31 @@ def refine_image(model, p, i, kept, depth, hypotheses, out_dir, masks=None):
              im_id=np.asarray(kept.infos.view_id).astype(np.int32), object_id=labels, time=coarse_time,
              refinement_time=np.full(n, start.elapsed_time(stop) / 1e3), poses=poses.cpu().numpy(),
              scores=scores.cpu().numpy(), hypothesis=refined.best_hypothesis.cpu().numpy(),
-             icp_status=status.cpu().numpy())
+             **{status_key: status.cpu().numpy()})
     return refined
 
 
 @torch.no_grad()
 def run(model, dataset_dir, out_dir, setting="localization", detections=None, template_poses=None, run_id="bop_run",
-        dataset_name=None, refine_hypotheses=0, refine_masks=False):
+        dataset_name=None, refine_hypotheses=0, refine_masks=False, depth_refiner="icp"):
     """Runs the test split: onboards the dataset from `template_poses` unless the model already holds it, then one
     `eval_retrieval` per image (predictions under out_dir/predictions, which must hold no .npz yet) and the csv.
     -> path of the csv (`{model}-pbrreal-rgb-mmodel_{dataset}-test_{run_id}.csv` in out_dir/predictions).
     With `refine_hypotheses` = H in 1 .. k, each image's kept instances also go through `refine_image` with the image's
     depth PNG, and a second csv (`..._{run_id}_icp.csv` in out_dir/refined_predictions) is written
     -> (coarse csv, refined csv).  With `refine_masks` they refine with their own CNOS masks (`refine_image`'s masks)
-    and the second csv is `..._{run_id}_icp_masked.csv`."""
+    and the second csv is `..._{run_id}_icp_masked.csv`.  With `depth_refiner="teaserpp"` (row f13) they go through
+    the TEASER++ refiner instead and the second csv is `..._{run_id}_teaserpp.csv`; it takes no masks."""
     from src.utils.inout import save_predictions_from_batched_predictions
     H = int(refine_hypotheses)
     if not 0 <= H <= model.testing_metric.k:
         raise BopRunError(f"refine_hypotheses {H} outside [0, {model.testing_metric.k}]")
     if refine_masks and not H:
         raise BopRunError("refine_masks needs refine_hypotheses >= 1")
+    if depth_refiner not in ("icp", "teaserpp"):
+        raise BopRunError(f"depth_refiner must be 'icp' or 'teaserpp', got {depth_refiner!r}")
+    if depth_refiner == "teaserpp" and refine_masks:
+        raise BopRunError("the teaserpp depth refiner takes no masks (refine_masks)")
     p = plan(dataset_dir, setting, detections, dataset_name, depth=H > 0)
     pred_dir, ref_dir = os.path.join(out_dir, "predictions"), os.path.join(out_dir, "refined_predictions")
     os.makedirs(pred_dir, exist_ok=True)
@@ -515,7 +528,7 @@ def run(model, dataset_dir, out_dir, setting="localization", detections=None, te
             selected, kept = model.eval_retrieval(batch, idx_batch=i, dataset_name=name)
             if H:
                 refine_image(model, p, i, kept, depth, H, out_dir,
-                             select_rle(batch.rle, selected) if refine_masks else None)
+                             select_rle(batch.rle, selected) if refine_masks else None, depth_refiner)
     finally:
         pre.close()
     stem = f"{model.model_name}-pbrreal-rgb-mmodel_{name}-test_{run_id}"
@@ -524,7 +537,7 @@ def run(model, dataset_dir, out_dir, setting="localization", detections=None, te
     coarse = os.path.join(pred_dir, f"{stem}.csv")
     if not H:
         return coarse
-    suffix = "_icp_masked" if refine_masks else "_icp"
+    suffix = "_teaserpp" if depth_refiner == "teaserpp" else "_icp_masked" if refine_masks else "_icp"
     save_predictions_from_batched_predictions(ref_dir, dataset_name=name, model_name=model.model_name,
                                               run_id=f"{run_id}{suffix}", is_refined=True)
     return coarse, os.path.join(ref_dir, f"{stem}{suffix}.csv")
@@ -555,6 +568,9 @@ def parser():
     ap.add_argument("--refine-masks", action="store_true",
                     help="with --refine-depth: refine each instance with its own CNOS mask, target normals smoothed "
                          "within it (writes ..._icp_masked.csv)")
+    ap.add_argument("--depth-refiner", choices=("icp", "teaserpp"), default="icp",
+                    help="with --refine-depth: the point-to-plane ICP (..._icp.csv) or MegaPose's TEASER++ refiner "
+                         "(..._teaserpp.csv, no masks)")
     ap.add_argument("--evaluate", action="store_true", help="score the csv (both, coarse first, when refining) with bop_eval")
     ap.add_argument("--device", default="cuda")
     return ap
@@ -564,9 +580,11 @@ def main(argv=None):
     a = parser().parse_args(argv)
     if a.refine_masks and not a.refine_depth:
         parser().error("--refine-masks needs --refine-depth H")
+    if a.depth_refiner == "teaserpp" and a.refine_masks:
+        parser().error("--depth-refiner teaserpp takes no --refine-masks")
     model = build_model(a.device, a.out, checkpoint=a.checkpoint)
     csvs = run(model, a.dataset_dir, a.out, a.setting, a.detections, a.template_poses, refine_hypotheses=a.refine_depth,
-               refine_masks=a.refine_masks)
+               refine_masks=a.refine_masks, depth_refiner=a.depth_refiner)
     csvs = (csvs,) if isinstance(csvs, str) else csvs
     for csv, out in zip(csvs, (a.out, os.path.join(a.out, "refined"))):
         print(csv)

@@ -8,9 +8,11 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libgigapose_b200.so")
-SOURCES = ["runtime.cu", "api.cu", "sim_search.cu", "prep.cu", "ist_mlp.cu", "ransac_pose.cu", "vit_gemm.cu", "vit_ops.cu", "vit_attention_tc.cu", "vit_api.cu", "ist_trunk.cu", "preprocess.cu", "render.cu", "depth_icp.cu", "depth_score.cu", "bop_eval.cu"]
+SOURCES = ["runtime.cu", "api.cu", "sim_search.cu", "prep.cu", "ist_mlp.cu", "ransac_pose.cu", "vit_gemm.cu", "vit_ops.cu", "vit_attention_tc.cu", "vit_api.cu", "ist_trunk.cu", "preprocess.cu", "render.cu", "depth_icp.cu", "depth_score.cu", "bop_eval.cu", "depth_teaser.cu"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
               "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr"]
+# sources whose contract states every floating-point operation rounds once (no multiply-add contraction)
+SOURCE_FLAGS = {"depth_teaser.cu": ["-fmad=false"]}
 
 
 def _nvcc() -> str:
@@ -36,7 +38,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
     os.makedirs(os.path.join(HERE, "build"), exist_ok=True)
     for src in SOURCES:
         obj = os.path.join(HERE, "build", src.replace(".cu", ".o"))
-        cmd = [_nvcc(), *NVCC_FLAGS, "-c", os.path.join(CSRC, src), "-o", obj]
+        cmd = [_nvcc(), *NVCC_FLAGS, *SOURCE_FLAGS.get(src, []), "-c", os.path.join(CSRC, src), "-o", obj]
         if verbose:
             cmd.insert(1, "-Xptxas=-v")
         procs.append((src, subprocess.Popen(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)))

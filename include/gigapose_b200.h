@@ -502,6 +502,71 @@ int gp_icp_refine_masked(int n_frames, int height, int width, const gp_icp_mask_
  * 0 <= rank < n; arguments are checked before any device work. */
 int gp_debug_icp_select(const uint32_t* bits, int n, int rank, uint32_t* out, void* stream);
 
+/* --- row f13: depth refinement with MegaPose's TeaserppRefiner (src/megapose/inference/teaserpp_refiner.py:165-291):
+ * pixel-aligned correspondences, farthest-point sampled, an exact maximum clique of the pairwise-consistency graph,
+ * GNC-TLS rotation and voted translation.  The full contract is the header comment of
+ * gigapose_b200/csrc/depth_teaser.cu.  Needs no handle. --------------------------------------------------------- */
+#define GP_TEASER_MAX_POINTS 1024
+#define GP_TEASER_OK 0                 /* solved and at least min_inliers inliers: [R|t] T0 written */
+#define GP_TEASER_TOO_FEW_POINTS 1     /* fewer than min_points masked pixels: T0 returned */
+#define GP_TEASER_CLIQUE_TOO_SMALL 2   /* maximum clique of fewer than 3 correspondences: T0 returned */
+#define GP_TEASER_CLIQUE_BUDGET 3      /* the clique search visited clique_budget nodes without finishing: T0 returned */
+#define GP_TEASER_TOO_FEW_INLIERS 4    /* fewer than min_inliers samples within noise_bound after the solve: T0 */
+#define GP_TEASER_INVALID 5            /* frame_idx outside [0, n_frames): T0 returned */
+
+/* One GNC-TLS iteration of one hypothesis (gp_teaser_debug_t.gnc), 112 bytes. */
+typedef struct gp_teaser_gnc {
+  int32_t iteration;             /* 0-based */
+  int32_t members;               /* clique size m = number of chain TIMs */
+  int32_t stopped;               /* 1: the mu initialisation ended the loop (mu not > 0 or not finite) */
+  int32_t reserved;              /* 0 */
+  double mu;                     /* the mu of this iteration's thresholds (at iteration 0 the initialised value) */
+  double cost;                   /* sum of the updated weights x residuals (0 when stopped) */
+  double max_residual;           /* largest squared TIM residual under R */
+  double R[9];                   /* the rotation solved with this iteration's weights, row-major */
+} gp_teaser_gnc_t;
+
+typedef struct gp_teaser_debug { /* every field nullable; test and timing hooks */
+  int32_t* counts;               /* [n_hyp,4] masked points N (-1: invalid frame), samples M, clique-search nodes,
+                                    GNC iterations */
+  float* points;                 /* [n_hyp,H*W,6] compacted (source xyz, target xyz), first N rows */
+  int32_t* samples;              /* [n_hyp,n_points] sampled point indices, first M entries */
+  uint32_t* adjacency;           /* [n_hyp,n_points,32] consistency graph rows of the samples, first M rows */
+  int32_t* clique;               /* [n_hyp,n_points] clique members (sample indices) ascending, -1 after the last */
+  gp_teaser_gnc_t* gnc;          /* [n_hyp,gnc_capacity] per-iteration records; iterations past it are not written */
+  double* gnc_weights;           /* [n_hyp,gnc_capacity,n_points] the weights each iteration's rotation used; needs gnc */
+  int32_t gnc_capacity;
+  int32_t stop_after;            /* timing: 0 runs everything; 1 compaction, 2 + sampling, 3 + graph and order, 4 + clique
+                                    only, with status -1 and T0 written where a hypothesis got that far */
+  double* transform;             /* [n_hyp,12] the solved R (row-major) and t, where the solve ran */
+} gp_teaser_debug_t;
+
+typedef struct gp_teaser_params {
+  float unit_per_m;              /* depth / translation units per metre (1000 for BOP's mm) */
+  int32_t min_points;            /* n_min_points, 100 (teaserpp_refiner.py:172) */
+  int32_t n_points;              /* samples, 1000 (n_points); 3 .. GP_TEASER_MAX_POINTS */
+  float noise_bound;             /* metres, 0.01 */
+  float cbar2;                   /* 1 */
+  int32_t min_inliers;           /* 50 */
+  float gnc_factor;              /* rotation_gnc_factor, 1.4 */
+  int32_t gnc_max_iters;         /* rotation_max_iterations, 100 */
+  double gnc_cost_threshold;     /* rotation_cost_threshold in m^2, 1e-12 (scaled by unit_per_m^2) */
+  int64_t clique_budget;         /* clique-search nodes before GP_TEASER_CLIQUE_BUDGET (the reference has no limit) */
+  gp_teaser_debug_t debug;
+} gp_teaser_params_t;
+
+/* Workspace bytes for n_hyp hypotheses of height x width: 28 B per hypothesis pixel plus 260 KiB per hypothesis. */
+int gp_teaser_query_sizes(int n_hyp, int height, int width, size_t* workspace_bytes);
+/* Per hypothesis: frame_idx i32 [n_hyp], depth f32 [n_frames,H,W] measured (not > 0 = missing), rendered_depth f32
+ * [n_hyp,H,W] and boxes i64 [n_hyp,4] from gp_render_templates at T0 f32 [n_hyp,4,4] with the frame's K f32
+ * [n_frames,3,3].  Outputs: out_poses f32 [n_hyp,4,4] (T0 bit for bit unless the status is GP_TEASER_OK),
+ * out_status i32, out_inliers i32 (0 where the solve did not run), out_clique i32 (the clique size, 0 where the search
+ * did not run; the best found so far on GP_TEASER_CLIQUE_BUDGET).  Three launches. */
+int gp_teaser_refine(int n_frames, int n_hyp, int height, int width, const int32_t* frame_idx, const float* depth,
+                     const float* rendered_depth, const int64_t* boxes, const float* T0, const float* K,
+                     const gp_teaser_params_t* params, float* out_poses, int32_t* out_status, int32_t* out_inliers,
+                     int32_t* out_clique, void* workspace, void* stream);
+
 /* --- row f10: depth-consistency score of the hypotheses of each detection, and the best one.  The full contract is the
  * header comment of gigapose_b200/csrc/depth_score.cu.  Needs no handle. ------------------------------------------ */
 /* frame_idx i32 [n_det]; depth f32 [n_frames,H,W] measured (not > 0 = missing); rendered f32 [n_det*n_hyp,H,W] the

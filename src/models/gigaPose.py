@@ -280,7 +280,7 @@ class GigaPose(LightningModule):
 
     @torch.no_grad()
     def refine_depth(self, dataset_name, predictions, depth, frame_idx=None, masks=None, hypotheses=1, *, K=None,
-                     rank=False, mask_normals=False, **params):
+                     rank=False, mask_normals=False, refiner="icp", **params):
         """MegaPose's ICPRefiner.refine_poses on the output of `retrieve()`: the first `hypotheses` of the k poses of every
         detection are rendered and refined against the measured depth (gigapose_b200.icp.refine_icp).
 
@@ -300,10 +300,19 @@ class GigaPose(LightningModule):
         With `mask_normals=True` (row f11, an extension: the reference smooths the whole frame) `masks` is required, one
         per detection, not per hypothesis: dense [B,H,W] or dict(counts=, offsets=) of COCO run-length masks
         (offsets [B+1], bop_run's layout); every hypothesis is refined against target normals smoothed within its
-        detection's mask (gigapose_b200.icp.refine_icp_masked)."""
+        detection's mask (gigapose_b200.icp.refine_icp_masked).
+
+        With `refiner="teaserpp"` (row f13) the hypotheses go through MegaPose's TeaserppRefiner instead
+        (gigapose_b200.teaser.refine_teaserpp, params as gigapose_b200.teaser.DEFAULTS) and the collection carries
+        `teaser_status`, `teaser_inliers` and `teaser_clique` [B,hypotheses] in place of the ICP's three; `rank` works
+        the same.  The reference's TEASER++ refiner takes no masks, so `masks` and `mask_normals` are refused with it."""
         from gigapose_b200.icp import DEFAULTS, refine_icp, refine_icp_masked, score_hypotheses
         if K is None:
             raise TypeError("refine_depth needs K=, the frames' full-image intrinsics [F,3,3] or [3,3]")
+        if refiner not in ("icp", "teaserpp"):
+            raise ValueError(f"refiner must be 'icp' or 'teaserpp', got {refiner!r}")
+        if refiner == "teaserpp" and (masks is not None or mask_normals):
+            raise ValueError("refiner='teaserpp' takes no masks: the reference's TEASER++ refiner ignores them")
         meshes = self.meshes[dataset_name]
         poses = predictions.pred_poses
         B, k = poses.shape[:2]
@@ -319,7 +328,12 @@ class GigaPose(LightningModule):
                 raise ValueError("frame_idx is needed when depth holds several frames")
         frame_idx = np.asarray(torch.as_tensor(frame_idx).cpu()).reshape(-1)
         labels = object_indices(predictions.infos, len(meshes))
-        if mask_normals:
+        if refiner == "teaserpp":
+            from gigapose_b200.teaser import refine_teaserpp
+            out, status, inliers, clique = refine_teaserpp(meshes, np.repeat(labels, h), poses[:, :h].reshape(-1, 4, 4),
+                                                           depth, K, np.repeat(frame_idx, h), **params)
+            extra = dict(teaser_status=status, teaser_inliers=inliers, teaser_clique=clique)
+        elif mask_normals:
             if masks is None:
                 raise ValueError("mask_normals=True needs masks, dense [B,H,W] or dict(counts=, offsets=)")
             dense, rle = (None, (masks["counts"], masks["offsets"])) if isinstance(masks, dict) else (masks, None)
@@ -331,14 +345,15 @@ class GigaPose(LightningModule):
                 masks = torch.as_tensor(masks).to(poses.device).repeat_interleave(h, 0)
             out, status, residual, fitness = refine_icp(meshes, np.repeat(labels, h), poses[:, :h].reshape(-1, 4, 4),
                                                         depth, K, np.repeat(frame_idx, h), masks, **params)
+        if refiner == "icp":
+            extra = dict(icp_status=status, icp_residual=residual, icp_fitness=fitness)
         refined = predictions.clone()
         refined.register_tensor("poses_input", poses.clone())
         new = poses.clone()
         new[:, :h] = out.reshape(B, h, 4, 4)
         refined.register_tensor("pred_poses", new)
-        refined.register_tensor("icp_status", status.reshape(B, h))
-        refined.register_tensor("icp_residual", residual.reshape(B, h))
-        refined.register_tensor("icp_fitness", fitness.reshape(B, h))
+        for name, v in extra.items():
+            refined.register_tensor(name, v.reshape(B, h))
         if rank:
             counts, score, best = score_hypotheses(meshes, np.repeat(labels, h), out, depth, K, np.repeat(frame_idx, h), h,
                                                    unit_per_m=params.get("unit_per_m", DEFAULTS["unit_per_m"]))
