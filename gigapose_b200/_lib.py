@@ -25,6 +25,8 @@ BOP_MAX_RECALL = 128           # GP_BOP_MAX_RECALL
 BOP_MATCH_GROUP_BYTES = 32     # GP_BOP_MATCH_GROUP_BYTES
 BOP_LABEL_FP, BOP_LABEL_TP, BOP_LABEL_IGNORED = 0, 1, 2          # GP_BOP_LABEL_*
 BOP_ADD_CHUNK = 1024           # GP_BOP_ADD_CHUNK
+VIS_CROP = 224                 # GP_VIS_CROP
+VIS_MAX_SIDE = 16384           # GP_VIS_MAX_SIDE
 
 
 class GpConfig(C.Structure):
@@ -189,6 +191,13 @@ SYMBOLS = {
                                            C.c_void_p]),
     "gp_bop_add": (C.c_int, [C.c_int, C.c_int, C.c_void_p, C.POINTER(C.c_int32), C.c_void_p, C.c_int, C.c_void_p,
                              C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "gp_vis_vertex_errors": (C.c_int, [C.c_int, C.c_int, C.c_void_p, C.POINTER(C.c_int32), C.c_void_p, C.c_void_p,
+                                       C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "gp_vis_heat_colors": (C.c_int, [C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_float, C.c_void_p, C.c_void_p]),
+    "gp_vis_overlay": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                 C.c_void_p]),
+    "gp_vis_kabsch": (C.c_int, [C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                C.c_void_p]),
     "gp_icp_query_sizes": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_size_t)]),
     "gp_icp_prepare_scene": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_float, C.c_void_p,
                                        C.c_void_p]),

@@ -483,7 +483,7 @@ def refine_image(model, p, i, kept, depth, hypotheses, out_dir, masks=None, refi
 
 @torch.no_grad()
 def run(model, dataset_dir, out_dir, setting="localization", detections=None, template_poses=None, run_id="bop_run",
-        dataset_name=None, refine_hypotheses=0, refine_masks=False, depth_refiner="icp"):
+        dataset_name=None, refine_hypotheses=0, refine_masks=False, depth_refiner="icp", vis_every=0):
     """Runs the test split: onboards the dataset from `template_poses` unless the model already holds it, then one
     `eval_retrieval` per image (predictions under out_dir/predictions, which must hold no .npz yet) and the csv.
     -> path of the csv (`{model}-pbrreal-rgb-mmodel_{dataset}-test_{run_id}.csv` in out_dir/predictions).
@@ -491,7 +491,9 @@ def run(model, dataset_dir, out_dir, setting="localization", detections=None, te
     depth PNG, and a second csv (`..._{run_id}_icp.csv` in out_dir/refined_predictions) is written
     -> (coarse csv, refined csv).  With `refine_masks` they refine with their own CNOS masks (`refine_image`'s masks)
     and the second csv is `..._{run_id}_icp_masked.csv`.  With `depth_refiner="teaserpp"` (row f13) they go through
-    the TEASER++ refiner instead and the second csv is `..._{run_id}_teaserpp.csv`; it takes no masks."""
+    the TEASER++ refiner instead and the second csv is `..._{run_id}_teaserpp.csv`; it takes no masks.
+    With `vis_every` = N > 0 (row f14) every N-th image's retrieval panels (`GigaPose.vis_retrieval`) are written to
+    out_dir/retrieved_sample_{i}.png, one row per rank and one column per kept detection, as the reference does."""
     from src.utils.inout import save_predictions_from_batched_predictions
     H = int(refine_hypotheses)
     if not 0 <= H <= model.testing_metric.k:
@@ -526,6 +528,10 @@ def run(model, dataset_dir, out_dir, setting="localization", detections=None, te
             rgb, depth = pre.get(i)
             batch = image_batch(p, i, rgb, device)
             selected, kept = model.eval_retrieval(batch, idx_batch=i, dataset_name=name)
+            if vis_every and i % vis_every == 0 and len(selected):
+                from torchvision.utils import save_image
+                save_image(model.vis_retrieval(name, batch, kept, selected),
+                           os.path.join(out_dir, f"retrieved_sample_{i}.png"), nrow=len(selected))
             if H:
                 refine_image(model, p, i, kept, depth, H, out_dir,
                              select_rle(batch.rle, selected) if refine_masks else None, depth_refiner)
@@ -571,6 +577,8 @@ def parser():
     ap.add_argument("--depth-refiner", choices=("icp", "teaserpp"), default="icp",
                     help="with --refine-depth: the point-to-plane ICP (..._icp.csv) or MegaPose's TEASER++ refiner "
                          "(..._teaserpp.csv, no masks)")
+    ap.add_argument("--vis-every", type=int, default=0, metavar="N",
+                    help="write the retrieval panels of every N-th image to <out>/retrieved_sample_<i>.png (0: none)")
     ap.add_argument("--evaluate", action="store_true", help="score the csv (both, coarse first, when refining) with bop_eval")
     ap.add_argument("--device", default="cuda")
     return ap
@@ -584,7 +592,7 @@ def main(argv=None):
         parser().error("--depth-refiner teaserpp takes no --refine-masks")
     model = build_model(a.device, a.out, checkpoint=a.checkpoint)
     csvs = run(model, a.dataset_dir, a.out, a.setting, a.detections, a.template_poses, refine_hypotheses=a.refine_depth,
-               refine_masks=a.refine_masks, depth_refiner=a.depth_refiner)
+               refine_masks=a.refine_masks, depth_refiner=a.depth_refiner, vis_every=a.vis_every)
     csvs = (csvs,) if isinstance(csvs, str) else csvs
     for csv, out in zip(csvs, (a.out, os.path.join(a.out, "refined"))):
         print(csv)

@@ -401,23 +401,42 @@ struct VertexTable {                  // host offsets, by value: object o owns v
   int32_t off[GP_BOP_MAX_OBJECTS + 1];
 };
 
+// Row f14 (gp_vis_vertex_errors, csrc/vis.cu) runs the same kernel with kPerVertex = true: no projection, and instead of
+// the chunk partials it stores each ground-truth vertex's ADD distance (symmetric[pair] = 0) or ADD-S distance (!= 0)
+// at values[out_off[pair] + j].  A pair whose object index is out of range, or whose slot out_off[pair + 1] -
+// out_off[pair] is not the object's vertex count, gets NaN over the part of its slot that the grid covers.
+template <bool kPerVertex>
 __global__ void __launch_bounds__(kThreads, 2)
 add_kernel(int n_objects, const int32_t* __restrict__ obj_idx, VertexTable tab, const float* __restrict__ vertices,
            int n_frames, const float* __restrict__ Kmat, const int32_t* __restrict__ frame_idx,
-           const float* __restrict__ pose_est, const float* __restrict__ pose_gt, double* __restrict__ partial) {
+           const float* __restrict__ pose_est, const float* __restrict__ pose_gt, double* __restrict__ partial,
+           const uint8_t* __restrict__ symmetric, const long long* __restrict__ out_off, float* __restrict__ values) {
   __shared__ float4 sE[kAddTile];
-  __shared__ float sDist[3][GP_BOP_ADD_CHUNK];
+  __shared__ float sDist[3][kPerVertex ? 1 : GP_BOP_ADD_CHUNK];
   __shared__ float sPe[16], sPg[16], sK[9];
   const int pair = blockIdx.x, chunk = blockIdx.y, tid = threadIdx.x;
-  const int o = obj_idx[pair], f = frame_idx[pair];
-  if (o < 0 || o >= n_objects || f < 0 || f >= n_frames) return;   // add_finish_kernel writes NaN
-  const int v0 = tab.off[o], n = tab.off[o + 1] - v0;
+  const int o = obj_idx[pair], f = kPerVertex ? 0 : frame_idx[pair];
   const int j0 = chunk * GP_BOP_ADD_CHUNK;
+  if constexpr (kPerVertex) {
+    const long long s0 = out_off[pair], len = out_off[pair + 1] - s0;
+    if (o < 0 || o >= n_objects || len != tab.off[o + 1] - tab.off[o]) {
+      for (int r = 0; r < kAddPerThread; ++r) {
+        const long long j = j0 + tid + kThreads * r;
+        if (j < len) values[s0 + j] = __int_as_float(0x7fffffff);
+      }
+      return;
+    }
+  } else if (o < 0 || o >= n_objects || f < 0 || f >= n_frames) {
+    return;                                                  // add_finish_kernel writes NaN
+  }
+  const int v0 = tab.off[o], n = tab.off[o + 1] - v0;
   if (j0 >= n) return;
+  const bool min_needed = !kPerVertex || symmetric[pair];
   if (tid < 16) { sPe[tid] = pose_est[16 * (size_t)pair + tid]; sPg[tid] = pose_gt[16 * (size_t)pair + tid]; }
-  if (tid < 9) sK[tid] = Kmat[9 * (size_t)f + tid];
+  if (!kPerVertex && tid < 9) sK[tid] = Kmat[9 * (size_t)f + tid];
   __syncthreads();
   float g[kAddPerThread][3];
+  float add[kAddPerThread];
   unsigned best[kAddPerThread];
 #pragma unroll
   for (int r = 0; r < kAddPerThread; ++r) {
@@ -426,20 +445,24 @@ add_kernel(int n_objects, const int32_t* __restrict__ obj_idx, VertexTable tab, 
     if (j < n) {
       const float* p = vertices + 3 * (size_t)(v0 + j);
       const float x = p[0], y = p[1], z = p[2];
-      float e[3], ue, ve, ug, vg;
+      float e[3];
       affine(sPe, x, y, z, e);
       affine(sPg, x, y, z, g[r]);
-      project(sK, e, ue, ve);
-      project(sK, g[r], ug, vg);
-      const float du = __fsub_rn(ue, ug), dv = __fsub_rn(ve, vg);
-      sDist[0][tid + kThreads * r] =
-          __fsqrt_rn(sq3(__fsub_rn(e[0], g[r][0]), __fsub_rn(e[1], g[r][1]), __fsub_rn(e[2], g[r][2])));
-      sDist[2][tid + kThreads * r] = __fsqrt_rn(__fadd_rn(__fmul_rn(du, du), __fmul_rn(dv, dv)));
+      add[r] = __fsqrt_rn(sq3(__fsub_rn(e[0], g[r][0]), __fsub_rn(e[1], g[r][1]), __fsub_rn(e[2], g[r][2])));
+      if constexpr (!kPerVertex) {
+        float ue, ve, ug, vg;
+        project(sK, e, ue, ve);
+        project(sK, g[r], ug, vg);
+        const float du = __fsub_rn(ue, ug), dv = __fsub_rn(ve, vg);
+        sDist[0][tid + kThreads * r] = add[r];
+        sDist[2][tid + kThreads * r] = __fsqrt_rn(__fadd_rn(__fmul_rn(du, du), __fmul_rn(dv, dv)));
+      }
     } else {
       g[r][0] = g[r][1] = g[r][2] = 0.f;
+      add[r] = 0.f;
     }
   }
-  for (int base = 0; base < n; base += kAddTile) {
+  for (int base = 0; min_needed && base < n; base += kAddTile) {   // min_needed is uniform over the CTA
     const int m = min(kAddTile, n - base);
     __syncthreads();                                         // the previous tile has been read
     for (int i = tid; i < m; i += kThreads) {
@@ -458,15 +481,24 @@ add_kernel(int n_objects, const int32_t* __restrict__ obj_idx, VertexTable tab, 
                                                    __fsub_rn(e.z, g[r][2]))));
     }
   }
+  if constexpr (kPerVertex) {
+    const long long s0 = out_off[pair];
 #pragma unroll
-  for (int r = 0; r < kAddPerThread; ++r)
-    if (j0 + tid + kThreads * r < n) sDist[1][tid + kThreads * r] = __fsqrt_rn(__uint_as_float(best[r]));
-  __syncthreads();
-  if (tid < 3) {
-    const int cnt = min(GP_BOP_ADD_CHUNK, n - j0);
-    double s = (double)sDist[tid][0];
-    for (int j = 1; j < cnt; ++j) s = __dadd_rn(s, (double)sDist[tid][j]);
-    partial[((size_t)pair * gridDim.y + chunk) * 3 + tid] = s;
+    for (int r = 0; r < kAddPerThread; ++r) {
+      const int j = j0 + tid + kThreads * r;
+      if (j < n) values[s0 + j] = min_needed ? __fsqrt_rn(__uint_as_float(best[r])) : add[r];
+    }
+  } else {
+#pragma unroll
+    for (int r = 0; r < kAddPerThread; ++r)
+      if (j0 + tid + kThreads * r < n) sDist[1][tid + kThreads * r] = __fsqrt_rn(__uint_as_float(best[r]));
+    __syncthreads();
+    if (tid < 3) {
+      const int cnt = min(GP_BOP_ADD_CHUNK, n - j0);
+      double s = (double)sDist[tid][0];
+      for (int j = 1; j < cnt; ++j) s = __dadd_rn(s, (double)sDist[tid][j]);
+      partial[((size_t)pair * gridDim.y + chunk) * 3 + tid] = s;
+    }
   }
 }
 
@@ -577,12 +609,27 @@ extern "C" int gp_bop_add(int n_pairs, int n_objects, const int32_t* obj_idx, co
   if (reinterpret_cast<uintptr_t>(workspace) % 8) return fail(GP_ERR_INVALID, "workspace must be 8-byte aligned");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   double* partial = static_cast<double*>(workspace);
-  GP_CUDA(gp::launch_ex(add_kernel, dim3(n_pairs, n_chunks), kThreads, 0, st, 1, false, n_objects, obj_idx, tab,
-                        vertices, n_frames, K, frame_idx, pose_est, pose_gt, partial));
+  GP_CUDA(gp::launch_ex(add_kernel<false>, dim3(n_pairs, n_chunks), kThreads, 0, st, 1, false, n_objects, obj_idx, tab,
+                        vertices, n_frames, K, frame_idx, pose_est, pose_gt, partial, nullptr, nullptr, nullptr));
   GP_CUDA(gp::launch_ex(add_finish_kernel, (unsigned)((3ll * n_pairs + kThreads - 1) / kThreads), kThreads, 0, st, 1,
                         false, n_pairs, n_chunks, n_objects, obj_idx, tab, n_frames, frame_idx,
                         static_cast<const double*>(partial), out));
   return GP_OK;
+}
+
+// gp_vis_vertex_errors (csrc/vis.cu) validates its arguments and launches add_kernel<true> through here
+cudaError_t gp::launch_add_vertex_errors(int n_pairs, int n_objects, const int32_t* obj_idx,
+                                         const int32_t* vertex_offsets, const float* vertices, const float* pose_est,
+                                         const float* pose_gt, const uint8_t* symmetric, const int64_t* out_offsets,
+                                         float* values, cudaStream_t st) {
+  VertexTable tab;
+  int max_v = 0;
+  for (int o = 0; o <= GP_BOP_MAX_OBJECTS; ++o) tab.off[o] = o <= n_objects ? vertex_offsets[o] : 0;
+  for (int o = 1; o <= n_objects; ++o) max_v = max(max_v, vertex_offsets[o] - vertex_offsets[o - 1]);
+  const int n_chunks = (max_v + GP_BOP_ADD_CHUNK - 1) / GP_BOP_ADD_CHUNK;
+  return gp::launch_ex(add_kernel<true>, dim3(n_pairs, n_chunks), kThreads, 0, st, 1, false, n_objects, obj_idx, tab,
+                       vertices, 1, nullptr, nullptr, pose_est, pose_gt, nullptr, symmetric,
+                       reinterpret_cast<const long long*>(out_offsets), values);
 }
 
 static bool check_offsets(const int32_t* off, int n) {

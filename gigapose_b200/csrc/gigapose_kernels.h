@@ -221,4 +221,11 @@ __device__ __forceinline__ bool rle_bit(const long long* __restrict__ ends, long
   return lo < r1 && ((lo - r0) & 1);
 }
 
+// ---------------------------------------------------------------- per-vertex ADD / ADD-S (bop_eval.cu, row f14)
+// add_kernel<true> over n_pairs pairs with the host vertex offsets already checked by the caller (gp_vis_vertex_errors).
+cudaError_t launch_add_vertex_errors(int n_pairs, int n_objects, const int32_t* obj_idx, const int32_t* vertex_offsets,
+                                     const float* vertices, const float* pose_est, const float* pose_gt,
+                                     const uint8_t* symmetric, const int64_t* out_offsets, float* values,
+                                     cudaStream_t s);
+
 }  // namespace gp

@@ -391,6 +391,36 @@ int gp_bop_add(int n_pairs, int n_objects, const int32_t* obj_idx, const int32_t
                int n_frames, const float* K, const int32_t* frame_idx, const float* pose_est, const float* pose_gt,
                void* workspace, double* out, void* stream);
 
+/* --- row f14: the reference's diagnostic images (vis_bop_results.py's overlays and error heat maps, plot_Kabsch's
+ * retrieval panels).  The full contract, with every rounding, is the header comment of gigapose_b200/csrc/vis.cu.
+ * Needs no handle; every pointer is device memory unless marked HOST. ------------------------------------------------ */
+#define GP_VIS_CROP 224              /* side of the retrieval crops of gp_vis_kabsch */
+#define GP_VIS_MAX_SIDE 16384        /* largest image side of gp_vis_overlay */
+/* Per-vertex error of n_pairs (estimate, ground truth) pairs, in gp_bop_add's tables (obj_idx, HOST vertex_offsets,
+ * vertices, pose_est, pose_gt; no frames): values f32 [out_offsets[n_pairs]], pair p's at [out_offsets[p],
+ * out_offsets[p + 1]) (i64 [n_pairs + 1]; the slot length is the vertex count of the pair's object), the ADD distance
+ * of each vertex, or the ADD-S distance (nearest estimated point of each ground-truth point) where symmetric u8
+ * [n_pairs] is nonzero.  A pair whose object index is out of range or whose slot length differs gets NaN.  One launch. */
+int gp_vis_vertex_errors(int n_pairs, int n_objects, const int32_t* obj_idx, const int32_t* vertex_offsets,
+                         const float* vertices, const float* pose_est, const float* pose_gt, const uint8_t* symmetric,
+                         const int64_t* out_offsets, float* values, void* stream);
+/* Heat-map vertex colours of n_pairs pairs from gp_vis_vertex_errors' values, offsets and symmetric flags:
+ * colors f32 [offsets[n_pairs], 3] in [0, 1] (turbo, normalised per pair over the values with max_distance appended,
+ * and 0 for a symmetric pair), for gp_render_templates' vertex_color.  max_distance > 0, in the unit of the values. */
+int gp_vis_heat_colors(int n_pairs, const int64_t* offsets, const uint8_t* symmetric, const float* values,
+                       float max_distance, float* colors, void* stream);
+/* Composites n_layers renders over one image: image u8 [H,W,3] (NULL = black) turned grey, then per layer in order
+ * its RGB where its alpha > 0 and, when colors u8 [n_layers,3] is not NULL, its contour in its colour.  renders f32
+ * [n_layers,4,H,W] and boxes i64 [n_layers,4] as gp_render_templates writes them.  Output out u8 [H,W,3]. */
+int gp_vis_overlay(int height, int width, int n_layers, const uint8_t* image, const float* renders,
+                   const int64_t* boxes, const uint8_t* colors, uint8_t* out, void* stream);
+/* Retrieval panels of n (query, template, M) triples: query / tmpl f32 [n,3,224,224] normalised crops, query_mask /
+ * tmpl_mask f32 [n,224,224], M f32 [n,3,3] (template crop -> query crop).  Output out u8 [n,224,224,3]: the query in
+ * grey with the template warped by M pasted through its warped mask, the warped mask's edge red and the query mask's
+ * edge green. */
+int gp_vis_kabsch(int n, const float* query, const float* query_mask, const float* tmpl, const float* tmpl_mask,
+                  const float* M, uint8_t* out, void* stream);
+
 /* --- row f6: depth refinement of the coarse poses (MegaPose's ICPRefiner, src/megapose/inference/icp_refiner.py:134-287,
  * with a GPU point-to-plane ICP in place of OpenCV's ppf_match_3d_ICP).  The full contract is the header comment of
  * gigapose_b200/csrc/depth_icp.cu.  Needs no handle. ------------------------------------------------------------- */

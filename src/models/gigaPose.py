@@ -35,6 +35,9 @@ class _HostResult:
         return self._poses, self._scores
 
 
+RENDERS_NOT_KEPT = "renders not kept"      # GigaPose.template_views entry of a bank built by onboard_templates
+
+
 def object_indices(infos, num_objects: int) -> np.ndarray:
     """0-based object indices from the `label` column (1-based ids as strings, gigaPose.py:514-520).  The reference
     indexes `template_data.ae_features[label - 1]`: label 0 silently wraps to the last object and label > O raises;
@@ -133,6 +136,9 @@ class GigaPose(LightningModule):
         # opt-in: replay the per-batch launch sequence (~250 kernels) as one CUDA graph per batch size
         self.use_cuda_graph = bool(kwargs.get("cuda_graph", False))
         self._graphs = {}
+        # row f14: how `template_crops` gets each dataset's template crops back: a view renderer after onboard_meshes,
+        # RENDERS_NOT_KEPT after onboard_templates, no entry after set_template_data (read from template_datasets)
+        self.template_views = {}
 
     # ------------------------------------------------------------------ out of scope: training
     def training_step(self, *a, **k):
@@ -196,6 +202,7 @@ class GigaPose(LightningModule):
         self.engines[dataset_name] = eng
         self.template_datas[dataset_name] = tc.PandasTensorCollection(infos=pd.DataFrame(), K=K, M=M, poses=P)
         self.pose_recovery[dataset_name] = ObjectPoseRecovery(template_K=K, template_Ms=M, template_poses=P)
+        self.template_views.pop(dataset_name, None)                 # template_crops reads template_datasets
         self.onboarding_s_per_object = start.elapsed_time(stop) / 1e3 / n_obj
         logger.info(f"Init {dataset_name} done! Avg time={self.onboarding_s_per_object:.3f} s/object")
 
@@ -209,8 +216,10 @@ class GigaPose(LightningModule):
         Crop + resize + pad (`CropResizePad`, utils/crop.py:16-61) and the CLIP normalisation of the RGB channels
         (template.py:71-73) run as one gather kernel per object (`gp_crop_resize_pad`); the crops then stream through the
         ViT / IST encoders in full 64-crop chunks across object boundaries into the bank."""
+        # the caller's renders are not kept: they can be [O,T,4,H,W] f32, gigabytes, and are freed with the caller's copy
         return self._onboard(dataset_name, len(rgba), rgba[0].shape[0],
-                             lambda o: (rgba[o].to(self.device, non_blocking=True).float(), boxes[o]), K, poses)
+                             lambda o: (rgba[o].to(self.device, non_blocking=True).float(), boxes[o]), K, poses,
+                             RENDERS_NOT_KEPT)
 
     @torch.no_grad()
     def onboard_meshes(self, dataset_name, meshes, poses, K=None):
@@ -228,15 +237,16 @@ class GigaPose(LightningModule):
         poses = torch.as_tensor(poses, dtype=torch.float32)
         poses = poses.expand(n_obj, *poses.shape[-3:]) if poses.dim() == 3 else poses
 
-        def produce(o):
+        def views(o, ids):
             mesh = read_ply(meshes[o]) if isinstance(meshes[o], (str, os.PathLike)) else meshes[o]
-            r = render_templates(mesh, poses[o].to(self.device), K, device=self.device)
+            r = render_templates(mesh, poses[o][ids].to(self.device), K, device=self.device)
             return r["rgba"], r["boxes"]
 
-        return self._onboard(dataset_name, n_obj, poses.shape[1], produce, K, poses)
+        return self._onboard(dataset_name, n_obj, poses.shape[1], lambda o: views(o, slice(None)), K, poses, views)
 
-    def _onboard(self, dataset_name, n_obj, T, produce, K, poses):
-        """The body of both onboarding entry points: `produce(o)` -> (rgba [T,4,H,W] f32 on the device, boxes [T,4])."""
+    def _onboard(self, dataset_name, n_obj, T, produce, K, poses, views):
+        """The body of both onboarding entry points: `produce(o)` -> (rgba [T,4,H,W] f32 on the device, boxes [T,4]);
+        `views(o, ids)` the same for the views `ids` only, kept for `template_crops` (or RENDERS_NOT_KEPT)."""
         from gigapose_b200.engine import Engine
         from gigapose_b200.preprocess import CLIP_MEAN, CLIP_STD, crop_resize_pad
         device = self.device
@@ -265,9 +275,60 @@ class GigaPose(LightningModule):
         self.engines[dataset_name] = eng
         self.template_datas[dataset_name] = tc.PandasTensorCollection(infos=pd.DataFrame(), K=K, M=M, poses=P)
         self.pose_recovery[dataset_name] = ObjectPoseRecovery(template_K=K, template_Ms=M, template_poses=P)
+        self.template_views[dataset_name] = views
         self.onboarding_s_per_object = start.elapsed_time(stop) / 1e3 / n_obj
         logger.info(f"Onboarded {dataset_name}: {n_obj} objects x {T} templates, {self.onboarding_s_per_object:.3f} s/object")
         return eng
+
+    # ------------------------------------------------------------------ row f14: retrieval panels (gigaPose.py:451-479)
+    @torch.no_grad()
+    def template_crops(self, dataset_name, obj, ids):
+        """The normalised template crops f32 [n,3,224,224] and masks f32 [n,224,224] of views `ids` of object index
+        `obj` (0-based) as the bank was built from them: read from `template_datasets` after `set_template_data`, and
+        re-rendered and re-cropped (the same `crop_resize_pad`) after `onboard_meshes`.  After `onboard_templates` the
+        caller's renders are not kept, so there is nothing to read them from: that raises ValueError."""
+        from gigapose_b200.preprocess import CLIP_MEAN, CLIP_STD, crop_resize_pad
+        ids = torch.as_tensor(np.asarray(ids, np.int64))
+        views = self.template_views.get(dataset_name)
+        if views is RENDERS_NOT_KEPT:
+            raise ValueError(f"{dataset_name} was onboarded from caller renders (onboard_templates), which are not kept: "
+                             "its template crops are not available; onboard it with onboard_meshes or set_template_data")
+        if views is None:
+            data = self.template_datasets[dataset_name][obj]
+            return data.rgb[ids].to(self.device).float(), data.mask[ids].to(self.device).float()
+        rgba, boxes = views(obj, ids)
+        crop = crop_resize_pad(torch.as_tensor(boxes), rgba, 224, mean=CLIP_MEAN + (0.0,), std=CLIP_STD + (1.0,))
+        return crop["images"][:, :3].contiguous(), crop["images"][:, 3].contiguous()
+
+    @torch.no_grad()
+    def vis_retrieval(self, dataset_name, batch, predictions, selected=None):
+        """The reference's retrieval panels (plot_Kabsch, src/libVis/torch.py) for the k retrieved templates of each
+        detection: the template warped by its predicted affine M onto the grey query crop, the warped mask's edge red
+        and the query mask's edge green (`gigapose_b200.vis.kabsch`; the keypoint panel is not drawn).  `predictions`
+        is what `eval_retrieval` returns for `batch`, `selected` its batch rows (default: all of them).
+        -> f32 [k * B, 3, 224, 224] in [0, 1], rank-major as the reference concatenates them."""
+        from gigapose_b200.vis import kabsch
+        eng = self.engines[dataset_name]
+        obj = object_indices(predictions.infos, eng.O)
+        B, k = predictions.id_src.shape[:2]
+        rows = torch.as_tensor(np.arange(B) if selected is None else np.asarray(selected, np.int64), device=eng.device)
+        tar_img, tar_mask = batch.tar_img.to(eng.device)[rows], batch.tar_mask.to(eng.device)[rows].float()
+        ids = predictions.id_src.long().cpu().numpy()
+        src_img = torch.empty(B, k, 3, 224, 224, device=eng.device)
+        src_mask = torch.empty(B, k, 224, 224, device=eng.device)
+        for o in np.unique(obj):
+            b = np.nonzero(obj == o)[0]
+            views, inv = np.unique(ids[b].reshape(-1), return_inverse=True)
+            rgb, mask = self.template_crops(dataset_name, int(o), views)
+            src_img[b] = rgb[inv].reshape(len(b), k, 3, 224, 224)
+            src_mask[b] = mask[inv].reshape(len(b), k, 224, 224)
+        M = predictions.M.float()
+        q = tar_img.float().unsqueeze(1).expand(B, k, 3, 224, 224).transpose(0, 1).reshape(k * B, 3, 224, 224)
+        qm = tar_mask.unsqueeze(1).expand(B, k, 224, 224).transpose(0, 1).reshape(k * B, 224, 224)
+        panels = kabsch(q.contiguous(), qm.contiguous(), src_img.transpose(0, 1).reshape(k * B, 3, 224, 224).contiguous(),
+                        src_mask.transpose(0, 1).reshape(k * B, 224, 224).contiguous(),
+                        M.transpose(0, 1).reshape(k * B, 3, 3).contiguous())
+        return panels.permute(0, 3, 1, 2).float() / 255.0
 
     # ------------------------------------------------------------------ row f6: depth refinement (icp_refiner.py:134-287)
     def attach_meshes(self, dataset_name, meshes):
