@@ -206,13 +206,23 @@ def xywh_to_xyxy(bbox):
     return np.stack([b[:, 0], b[:, 1], b[:, 0] + b[:, 2], b[:, 1] + b[:, 3]], 1).astype(np.int64)
 
 
-def image_inputs(dets, targets, dataset_name, shape, key):
+def image_inputs(dets, targets, dataset_name, shape, key, target_size=224):
     """One image's host inputs: labels (object ids, LM-O indices for lmo), i64 xyxy boxes, concatenated i32 RLE counts
-    and their offsets [n+1], the test list rows and the image's detection time (its first detection's)."""
+    and their offsets [n+1], the test list rows and the image's detection time (its first detection's).  A box whose
+    crop has no rows or columns once resized to target_size (a mask more than target_size times longer than it is
+    wide, or no pixel inside the image) is refused: the reference cannot crop it, and a crop of zeros would pass into
+    retrieval unnoticed."""
+    from .preprocess import empty_crops
     remap = (lambda o: LMO_ID_TO_INDEX[int(o)]) if "lmo" in dataset_name else int
     counts = [rle_counts(d["segmentation"], shape, f"image {key}, detection {i}") for i, d in enumerate(dets)]
+    boxes = xywh_to_xyxy([d["bbox"] for d in dets])
+    bad = empty_crops(boxes, shape[0], shape[1], target_size)
+    if len(bad):
+        i = int(bad[0])
+        raise BopRunError(f"image {key}, detection {i}: bbox {list(dets[i]['bbox'])} (xyxy {boxes[i].tolist()}) has "
+                          f"no rows or columns once resized to {target_size} x {target_size}; it cannot be cropped")
     return dict(labels=np.array([remap(d["category_id"]) for d in dets], np.int64),
-                boxes=xywh_to_xyxy([d["bbox"] for d in dets]),
+                boxes=boxes,
                 counts=np.concatenate(counts) if counts else np.zeros(0, np.int32),
                 offsets=np.concatenate([[0], np.cumsum([len(c) for c in counts])]).astype(np.int64),
                 obj_id=[remap(t["obj_id"]) for t in targets], inst_count=[int(t["inst_count"]) for t in targets],

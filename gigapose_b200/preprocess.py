@@ -17,6 +17,22 @@ CLIP_MEAN = (0.48145466, 0.4578275, 0.40821073)
 CLIP_STD = (0.26862954, 0.26130258, 0.27577711)
 
 
+def empty_crops(xyxy_boxes, height: int, width: int, target_size: int = 224) -> np.ndarray:
+    """Indices of the boxes whose crop is empty once resized, on the host: the box's part inside the image (corner
+    clamped to 0) has no rows or columns after `floor(size * scale)`, with the kernel's float32 scale
+    `T * (1 / max(w, h))`.  The reference cannot crop such a box (`F.interpolate` refuses an empty output); the kernel
+    writes zeros for it, so callers taking boxes from outside inputs refuse them with these indices."""
+    b = np.asarray(xyxy_boxes, np.int64).reshape(-1, 4)
+    x1, y1 = np.clip(b[:, 0], 0, width), np.clip(b[:, 1], 0, height)
+    cw = np.maximum(np.minimum(b[:, 2], width) - x1, 0)
+    ch = np.maximum(np.minimum(b[:, 3], height) - y1, 0)
+    side = np.maximum(b[:, 2] - b[:, 0], b[:, 3] - b[:, 1])
+    with np.errstate(divide="ignore", invalid="ignore"):
+        scale = (np.float32(1) / side.astype(np.float32)) * np.float32(target_size)     # __frcp_rn, __fmul_rn
+        short = np.floor(np.minimum(ch, cw).astype(np.float64) * scale.astype(np.float64))
+    return np.flatnonzero((side <= 0) | ~(short >= 1))
+
+
 @torch.no_grad()
 def crop_resize_pad(xyxy_boxes: torch.Tensor, images: torch.Tensor, target_size: int = 224,
                     image_index: Optional[torch.Tensor] = None, mask: Optional[torch.Tensor] = None, in_div: float = 1.0,
