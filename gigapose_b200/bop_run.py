@@ -23,9 +23,14 @@ Row f13, `--depth-refiner teaserpp` with `--refine-depth H`: the hypotheses go t
 (`GigaPose.refine_depth(refiner="teaserpp")`) instead of the ICP, with the same ranking; the csv is
 `..._{run_id}_teaserpp.csv`.  Usage:
 
-    python -m gigapose_b200.bop_run --dataset-dir D --checkpoint gigaPose_v1.ckpt --template-poses P.npy
+    python -m gigapose_b200.bop_run --dataset-dir D --checkpoint gigaPose_v1.ckpt
+        [--template-poses P.npy | [--template-level 0|1|2] [--pose-distribution all|upper]]
         [--setting localization|detection] [--detections FILE] [--out DIR]
         [--refine-depth H [--refine-masks | --depth-refiner teaserpp]] [--evaluate]
+
+Row f15: without --template-poses the templates are the reference's test templates, generated
+(`template_poses.template_poses`, level 1 and all views by default).  Under `torchrun --nproc-per-node N -m
+gigapose_b200.bop_run ...` each rank runs its share of the images on its own GPU (`main_ranks`).
 """
 from __future__ import annotations
 
@@ -491,20 +496,8 @@ def refine_image(model, p, i, kept, depth, hypotheses, out_dir, masks=None, refi
     return refined
 
 
-@torch.no_grad()
-def run(model, dataset_dir, out_dir, setting="localization", detections=None, template_poses=None, run_id="bop_run",
-        dataset_name=None, refine_hypotheses=0, refine_masks=False, depth_refiner="icp", vis_every=0):
-    """Runs the test split: onboards the dataset from `template_poses` unless the model already holds it, then one
-    `eval_retrieval` per image (predictions under out_dir/predictions, which must hold no .npz yet) and the csv.
-    -> path of the csv (`{model}-pbrreal-rgb-mmodel_{dataset}-test_{run_id}.csv` in out_dir/predictions).
-    With `refine_hypotheses` = H in 1 .. k, each image's kept instances also go through `refine_image` with the image's
-    depth PNG, and a second csv (`..._{run_id}_icp.csv` in out_dir/refined_predictions) is written
-    -> (coarse csv, refined csv).  With `refine_masks` they refine with their own CNOS masks (`refine_image`'s masks)
-    and the second csv is `..._{run_id}_icp_masked.csv`.  With `depth_refiner="teaserpp"` (row f13) they go through
-    the TEASER++ refiner instead and the second csv is `..._{run_id}_teaserpp.csv`; it takes no masks.
-    With `vis_every` = N > 0 (row f14) every N-th image's retrieval panels (`GigaPose.vis_retrieval`) are written to
-    out_dir/retrieved_sample_{i}.png, one row per rank and one column per kept detection, as the reference does."""
-    from src.utils.inout import save_predictions_from_batched_predictions
+def check_refine(model, refine_hypotheses, refine_masks, depth_refiner):
+    """-> H after checking the refinement options against the model's k."""
     H = int(refine_hypotheses)
     if not 0 <= H <= model.testing_metric.k:
         raise BopRunError(f"refine_hypotheses {H} outside [0, {model.testing_metric.k}]")
@@ -514,39 +507,68 @@ def run(model, dataset_dir, out_dir, setting="localization", detections=None, te
         raise BopRunError(f"depth_refiner must be 'icp' or 'teaserpp', got {depth_refiner!r}")
     if depth_refiner == "teaserpp" and refine_masks:
         raise BopRunError("the teaserpp depth refiner takes no masks (refine_masks)")
-    p = plan(dataset_dir, setting, detections, dataset_name, depth=H > 0)
+    return H
+
+
+def check_out(out_dir):
+    """Creates out_dir/predictions and refuses an out_dir whose prediction directories already hold .npz files."""
     pred_dir, ref_dir = os.path.join(out_dir, "predictions"), os.path.join(out_dir, "refined_predictions")
     os.makedirs(pred_dir, exist_ok=True)
     for d in (pred_dir, ref_dir):
         if glob.glob(os.path.join(glob.escape(d), "*.npz")):
             raise BopRunError(f"{d} already holds prediction files; use an empty --out")
+
+
+def prepare(model, dataset_dir, p, template_poses=None, template_level=1, pose_distribution="all", attach=False):
+    """Onboards the plan's dataset unless the model already holds it, from `template_poses` or, when that is None,
+    from the generated `template_poses.template_poses(template_level, pose_distribution)`; with `attach` (depth
+    refinement), attaches its meshes too."""
     name = p["name"]
-    attach = H > 0 and name not in getattr(model, "meshes", {})
-    if name not in model.engines and template_poses is None:
-        raise BopRunError(f"{name} is not onboarded and no template poses were given")
+    attach = attach and name not in getattr(model, "meshes", {})
     meshes = read_meshes(dataset_dir, name) if attach or name not in model.engines else None
     if name not in model.engines:
+        if template_poses is None:
+            from .template_poses import template_poses as generate
+            template_poses = generate(template_level, pose_distribution)
         onboard(model, dataset_dir, template_poses, name, meshes)
     if attach:
         model.attach_meshes(name, meshes)
+
+
+def run_images(model, p, indices, out_dir, H=0, refine_masks=False, depth_refiner="icp", vis_every=0):
+    """`eval_retrieval` (and, with H, `refine_image`) on the plan's images `indices`, each written under its index in
+    the plan, so that runs over disjoint shares of the images fill one out_dir.  An exception names its image in a
+    note."""
+    name = p["name"]
     model.log_dir = out_dir
     device = model.engines[name].device
-    pre = _Prefetch([image_path(dataset_dir, p["split"], s, im) for s, im in p["images"]],
-                    [(dataset_dir, p["split"], s, im, p["depth_scale"][s][im]) for s, im in p["images"]] if H else None)
+    images = [p["images"][i] for i in indices]
+    pre = _Prefetch([image_path(p["dataset_dir"], p["split"], s, im) for s, im in images],
+                    [(p["dataset_dir"], p["split"], s, im, p["depth_scale"][s][im]) for s, im in images] if H else None)
     try:
-        for i in range(len(p["images"])):
-            rgb, depth = pre.get(i)
-            batch = image_batch(p, i, rgb, device)
-            selected, kept = model.eval_retrieval(batch, idx_batch=i, dataset_name=name)
-            if vis_every and i % vis_every == 0 and len(selected):
-                from torchvision.utils import save_image
-                save_image(model.vis_retrieval(name, batch, kept, selected),
-                           os.path.join(out_dir, f"retrieved_sample_{i}.png"), nrow=len(selected))
-            if H:
-                refine_image(model, p, i, kept, depth, H, out_dir,
-                             select_rle(batch.rle, selected) if refine_masks else None, depth_refiner)
+        for n, i in enumerate(indices):
+            try:
+                rgb, depth = pre.get(n)
+                batch = image_batch(p, i, rgb, device)
+                selected, kept = model.eval_retrieval(batch, idx_batch=i, dataset_name=name)
+                if vis_every and i % vis_every == 0 and len(selected):
+                    from torchvision.utils import save_image
+                    save_image(model.vis_retrieval(name, batch, kept, selected),
+                               os.path.join(out_dir, f"retrieved_sample_{i}.png"), nrow=len(selected))
+                if H:
+                    refine_image(model, p, i, kept, depth, H, out_dir,
+                                 select_rle(batch.rle, selected) if refine_masks else None, depth_refiner)
+            except Exception as e:
+                e.add_note(f"while running image {i} (scene {images[n][0]}, image {images[n][1]})")
+                raise
     finally:
         pre.close()
+
+
+def write_csvs(model, name, out_dir, run_id="bop_run", H=0, refine_masks=False, depth_refiner="icp"):
+    """The csv(s) of the predictions under out_dir (see `run`)."""
+    from src.utils.inout import save_predictions_from_batched_predictions
+    pred_dir, ref_dir = os.path.join(out_dir, "predictions"), os.path.join(out_dir, "refined_predictions")
     stem = f"{model.model_name}-pbrreal-rgb-mmodel_{name}-test_{run_id}"
     save_predictions_from_batched_predictions(pred_dir, dataset_name=name, model_name=model.model_name,
                                               run_id=run_id, is_refined=False)
@@ -557,6 +579,76 @@ def run(model, dataset_dir, out_dir, setting="localization", detections=None, te
     save_predictions_from_batched_predictions(ref_dir, dataset_name=name, model_name=model.model_name,
                                               run_id=f"{run_id}{suffix}", is_refined=True)
     return coarse, os.path.join(ref_dir, f"{stem}{suffix}.csv")
+
+
+@torch.no_grad()
+def run(model, dataset_dir, out_dir, setting="localization", detections=None, template_poses=None, run_id="bop_run",
+        dataset_name=None, refine_hypotheses=0, refine_masks=False, depth_refiner="icp", vis_every=0,
+        template_level=1, pose_distribution="all"):
+    """Runs the test split: onboards the dataset unless the model already holds it, from `template_poses` ([T,4,4]
+    array or .npy path) or, when that is None, from the generated icosphere poses of `template_level` and
+    `pose_distribution` (`template_poses.template_poses`, the reference's test templates by default), then one
+    `eval_retrieval` per image (predictions under out_dir/predictions, which must hold no .npz yet) and the csv.
+    -> path of the csv (`{model}-pbrreal-rgb-mmodel_{dataset}-test_{run_id}.csv` in out_dir/predictions).
+    With `refine_hypotheses` = H in 1 .. k, each image's kept instances also go through `refine_image` with the image's
+    depth PNG, and a second csv (`..._{run_id}_icp.csv` in out_dir/refined_predictions) is written
+    -> (coarse csv, refined csv).  With `refine_masks` they refine with their own CNOS masks (`refine_image`'s masks)
+    and the second csv is `..._{run_id}_icp_masked.csv`.  With `depth_refiner="teaserpp"` (row f13) they go through
+    the TEASER++ refiner instead and the second csv is `..._{run_id}_teaserpp.csv`; it takes no masks.
+    With `vis_every` = N > 0 (row f14) every N-th image's retrieval panels (`GigaPose.vis_retrieval`) are written to
+    out_dir/retrieved_sample_{i}.png, one row per rank and one column per kept detection, as the reference does."""
+    H = check_refine(model, refine_hypotheses, refine_masks, depth_refiner)
+    p = plan(dataset_dir, setting, detections, dataset_name, depth=H > 0)
+    check_out(out_dir)
+    prepare(model, dataset_dir, p, template_poses, template_level, pose_distribution, attach=H > 0)
+    run_images(model, p, range(len(p["images"])), out_dir, H, refine_masks, depth_refiner, vis_every)
+    return write_csvs(model, p["name"], out_dir, run_id, H, refine_masks, depth_refiner)
+
+
+# ---------------------------------------------------------------------------------------------------- several ranks
+def shard_images(counts, world_size):
+    """Image indices per rank: greedy longest-first on the images' detection `counts` (the largest first, ties by image
+    index, each to the rank with the fewest detections so far, ties by rank), each share in image order.  No rank
+    ends more than the largest single count above the mean per rank."""
+    loads, shares = [0] * world_size, [[] for _ in range(world_size)]
+    for i in sorted(range(len(counts)), key=lambda i: (-counts[i], i)):
+        r = min(range(world_size), key=lambda r: (loads[r], r))
+        shares[r].append(i)
+        loads[r] += counts[i]
+    return [sorted(s) for s in shares]
+
+
+class RankFailed(RuntimeError):
+    pass
+
+
+class Ranks:
+    """The ranks of a `torchrun` launch on a gloo process group (env://).  `step(fn)` runs fn on this rank, then every
+    rank learns whether any rank raised: if one did, each raises `RankFailed` naming every failing rank and its error,
+    so no rank waits for one that has given up.  Each rank calls the same steps in the same order."""
+
+    def __init__(self):
+        import torch.distributed as dist
+        self.dist = dist
+        dist.init_process_group("gloo")
+        self.rank, self.world_size = dist.get_rank(), dist.get_world_size()
+
+    def step(self, fn, *args):
+        out, err = None, None
+        try:
+            out = fn(*args)
+        except Exception as e:
+            err = "".join([f"rank {self.rank}: {type(e).__name__}: {e}"] +
+                          [f"\n  {note}" for note in getattr(e, "__notes__", ())])
+        errors = [None] * self.world_size
+        self.dist.all_gather_object(errors, err)
+        failed = [e for e in errors if e is not None]
+        if failed:
+            raise RankFailed("\n".join(failed))
+        return out
+
+    def close(self):
+        self.dist.destroy_process_group()
 
 
 def _evaluate(csv, dataset_dir, setting, out_dir, device):
@@ -574,7 +666,13 @@ def parser():
     ap = argparse.ArgumentParser(description="GigaPose on a BOP test split with its CNOS detections -> BOP results csv")
     ap.add_argument("--dataset-dir", required=True, help="BOP dataset directory, e.g. <root>/lmo")
     ap.add_argument("--checkpoint", required=True, help="Lightning checkpoint (gigaPose_v1.ckpt)")
-    ap.add_argument("--template-poses", required=True, help="[T,4,4] .npy of template poses (see INTEGRATION.md)")
+    ap.add_argument("--template-poses", default=None,
+                    help="[T,4,4] .npy of template poses (see INTEGRATION.md); default: generated from --template-level "
+                         "and --pose-distribution")
+    ap.add_argument("--template-level", type=int, choices=(0, 1, 2), default=None,
+                    help="icosphere level of the generated template poses: 42, 162 or 642 views (default 1)")
+    ap.add_argument("--pose-distribution", choices=("all", "upper"), default=None,
+                    help="generated template poses: every view, or those whose camera has z >= 0 (default all)")
     ap.add_argument("--setting", choices=("localization", "detection"), default="localization")
     ap.add_argument("--detections", default=None, help="CNOS detections json (default: <root>/default_detections/...)")
     ap.add_argument("--out", default="bop_run_out")
@@ -600,14 +698,56 @@ def main(argv=None):
         parser().error("--refine-masks needs --refine-depth H")
     if a.depth_refiner == "teaserpp" and a.refine_masks:
         parser().error("--depth-refiner teaserpp takes no --refine-masks")
+    if a.template_poses is not None and (a.template_level is not None or a.pose_distribution is not None):
+        parser().error("--template-level and --pose-distribution choose generated template poses; "
+                       "they do not go with --template-poses")
+    a.template_level = 1 if a.template_level is None else a.template_level
+    a.pose_distribution = a.pose_distribution or "all"
+    if int(os.environ.get("WORLD_SIZE", "1")) > 1:
+        return main_ranks(a)
     model = build_model(a.device, a.out, checkpoint=a.checkpoint)
     csvs = run(model, a.dataset_dir, a.out, a.setting, a.detections, a.template_poses, refine_hypotheses=a.refine_depth,
-               refine_masks=a.refine_masks, depth_refiner=a.depth_refiner, vis_every=a.vis_every)
+               refine_masks=a.refine_masks, depth_refiner=a.depth_refiner, vis_every=a.vis_every,
+               template_level=a.template_level, pose_distribution=a.pose_distribution)
+    report(a, csvs, a.device)
+
+
+def report(a, csvs, device):
     csvs = (csvs,) if isinstance(csvs, str) else csvs
     for csv, out in zip(csvs, (a.out, os.path.join(a.out, "refined"))):
         print(csv)
         if a.evaluate:
-            _evaluate(csv, a.dataset_dir, a.setting, out, a.device)
+            _evaluate(csv, a.dataset_dir, a.setting, out, device)
+
+
+@torch.no_grad()
+def main_ranks(a):
+    """`main` under torchrun: every rank builds the model on cuda:LOCAL_RANK (or on --device when it names a device
+    index, so that several ranks can share one GPU), onboards the dataset itself and runs its `shard_images` share of
+    the plan's images into the same --out; rank 0 checks --out first and writes the csv(s) and scores last.  A rank
+    that fails makes every rank exit with its error (`Ranks.step`)."""
+    ranks = Ranks()
+    try:
+        device = torch.device(f"cuda:{os.environ.get('LOCAL_RANK', '0')}" if a.device == "cuda" else a.device)
+        if device.type == "cuda":
+            torch.cuda.set_device(device)
+        ranks.step(lambda: ranks.rank == 0 and check_out(a.out))
+
+        def work():
+            model = build_model(device, a.out, checkpoint=a.checkpoint)
+            H = check_refine(model, a.refine_depth, a.refine_masks, a.depth_refiner)
+            p = plan(a.dataset_dir, a.setting, a.detections, depth=H > 0)
+            prepare(model, a.dataset_dir, p, a.template_poses, a.template_level, a.pose_distribution, attach=H > 0)
+            counts = [len(p["detections"][_key(s, im)]) for s, im in p["images"]]
+            share = shard_images(counts, ranks.world_size)[ranks.rank]
+            run_images(model, p, share, a.out, H, a.refine_masks, a.depth_refiner, a.vis_every)
+            return model, p["name"], H
+
+        model, name, H = ranks.step(work)
+        ranks.step(lambda: ranks.rank == 0 and report(
+            a, write_csvs(model, name, a.out, "bop_run", H, a.refine_masks, a.depth_refiner), device))
+    finally:
+        ranks.close()
 
 
 if __name__ == "__main__":
