@@ -177,6 +177,10 @@ SYMBOLS = {
                                       C.c_float, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "gp_render_depth": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p,
                                   C.c_void_p, C.c_float, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "gp_recentre_boxes": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_void_p, C.POINTER(C.c_double),
+                                    C.POINTER(C.c_int64), C.c_void_p, C.c_void_p]),
+    "gp_recentre_crop": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.POINTER(C.c_double),
+                                   C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "gp_bop_vsd": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p,
                              C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_float,
                              C.c_int, C.POINTER(C.c_float), C.c_void_p, C.c_void_p, C.c_void_p]),

@@ -26,10 +26,16 @@ Row f13, `--depth-refiner teaserpp` with `--refine-depth H`: the hypotheses go t
     python -m gigapose_b200.bop_run --dataset-dir D --checkpoint gigaPose_v1.ckpt
         [--template-poses P.npy | [--template-level 0|1|2] [--pose-distribution all|upper]]
         [--setting localization|detection] [--detections FILE] [--out DIR]
-        [--refine-depth H [--refine-masks | --depth-refiner teaserpp]] [--evaluate]
+        [--refine-depth H [--refine-masks | --depth-refiner teaserpp]] [--onboarding models|static] [--evaluate]
 
 Row f15: without --template-poses the templates are the reference's test templates, generated
-(`template_poses.template_poses`, level 1 and all views by default).  Under `torchrun --nproc-per-node N -m
+(`template_poses.template_poses`, level 1 and all views by default).
+
+Row f16, `--onboarding static`: objects without CAD models.  The templates are built from the dataset's
+onboarding_static/ frames (`onboard_static`, `GigaPose.onboard_images`) for the same template viewpoints; models/ is
+not read, except models_info.json when it exists (to check the object ids) and by --evaluate, whose BOP metrics need
+the models.  The depth refiners render the CAD model, so --refine-depth is refused; the default run id is
+`bop_run_static`.  Under `torchrun --nproc-per-node N -m
 gigapose_b200.bop_run ...` each rank runs its share of the images on its own GPU (`main_ranks`).
 """
 from __future__ import annotations
@@ -349,6 +355,18 @@ def onboard(model, dataset_dir, template_poses, dataset_name=None, meshes=None):
     return model.onboard_meshes(name, meshes, torch.as_tensor(poses, dtype=torch.float32))
 
 
+def onboard_static(model, dataset_dir, template_poses, dataset_name=None):
+    """`GigaPose.onboard_images` on the dataset's onboarding_static/ frames (`onboarding.read_onboarding_static`) for
+    the [T,4,4] template poses (an .npy path or an array)."""
+    from .onboarding import read_onboarding_static
+    name = dataset_name or os.path.basename(os.path.normpath(dataset_dir))
+    poses = np.load(template_poses) if isinstance(template_poses, (str, os.PathLike)) else np.asarray(template_poses)
+    if poses.ndim != 3 or poses.shape[1:] != (4, 4):
+        raise BopRunError(f"template poses must be [T,4,4], got {poses.shape}")
+    frames = read_onboarding_static(dataset_dir)
+    return model.onboard_images(name, [frames[o] for o in sorted(frames)], poses)
+
+
 # ---------------------------------------------------------------------------------------------------- the loop
 def depth_path(dataset_dir, split, scene_id, im_id):
     """The depth PNG `bop_eval.load_depth` reads."""
@@ -519,11 +537,31 @@ def check_out(out_dir):
             raise BopRunError(f"{d} already holds prediction files; use an empty --out")
 
 
-def prepare(model, dataset_dir, p, template_poses=None, template_level=1, pose_distribution="all", attach=False):
+def check_onboarding(onboarding, H):
+    if onboarding not in ("models", "static"):
+        raise BopRunError(f"onboarding must be 'models' or 'static', got {onboarding!r}")
+    if onboarding == "static" and H:
+        raise BopRunError(STATIC_NO_DEPTH)
+
+
+STATIC_NO_DEPTH = ("--onboarding static takes no --refine-depth: the depth refiners render the CAD model, which "
+                   "model-free onboarding does not read")
+
+
+def prepare(model, dataset_dir, p, template_poses=None, template_level=1, pose_distribution="all", attach=False,
+            onboarding="models"):
     """Onboards the plan's dataset unless the model already holds it, from `template_poses` or, when that is None,
-    from the generated `template_poses.template_poses(template_level, pose_distribution)`; with `attach` (depth
+    from the generated `template_poses.template_poses(template_level, pose_distribution)`; from the CAD models, or
+    with onboarding="static" from the onboarding_static/ frames (`onboard_static`).  With `attach` (depth
     refinement), attaches its meshes too."""
     name = p["name"]
+    if onboarding == "static":
+        if name not in model.engines:
+            if template_poses is None:
+                from .template_poses import template_poses as generate
+                template_poses = generate(template_level, pose_distribution)
+            onboard_static(model, dataset_dir, template_poses, name)
+        return
     attach = attach and name not in getattr(model, "meshes", {})
     meshes = read_meshes(dataset_dir, name) if attach or name not in model.engines else None
     if name not in model.engines:
@@ -581,10 +619,14 @@ def write_csvs(model, name, out_dir, run_id="bop_run", H=0, refine_masks=False, 
     return coarse, os.path.join(ref_dir, f"{stem}{suffix}.csv")
 
 
+def default_run_id(onboarding="models"):
+    return "bop_run_static" if onboarding == "static" else "bop_run"
+
+
 @torch.no_grad()
-def run(model, dataset_dir, out_dir, setting="localization", detections=None, template_poses=None, run_id="bop_run",
+def run(model, dataset_dir, out_dir, setting="localization", detections=None, template_poses=None, run_id=None,
         dataset_name=None, refine_hypotheses=0, refine_masks=False, depth_refiner="icp", vis_every=0,
-        template_level=1, pose_distribution="all"):
+        template_level=1, pose_distribution="all", onboarding="models"):
     """Runs the test split: onboards the dataset unless the model already holds it, from `template_poses` ([T,4,4]
     array or .npy path) or, when that is None, from the generated icosphere poses of `template_level` and
     `pose_distribution` (`template_poses.template_poses`, the reference's test templates by default), then one
@@ -596,11 +638,17 @@ def run(model, dataset_dir, out_dir, setting="localization", detections=None, te
     and the second csv is `..._{run_id}_icp_masked.csv`.  With `depth_refiner="teaserpp"` (row f13) they go through
     the TEASER++ refiner instead and the second csv is `..._{run_id}_teaserpp.csv`; it takes no masks.
     With `vis_every` = N > 0 (row f14) every N-th image's retrieval panels (`GigaPose.vis_retrieval`) are written to
-    out_dir/retrieved_sample_{i}.png, one row per rank and one column per kept detection, as the reference does."""
+    out_dir/retrieved_sample_{i}.png, one row per rank and one column per kept detection, as the reference does.
+    With onboarding="static" (row f16) the templates come from the onboarding_static/ frames instead of the CAD
+    models (`onboard_static`), refinement is refused, and the default run_id is "bop_run_static" ("bop_run"
+    otherwise)."""
     H = check_refine(model, refine_hypotheses, refine_masks, depth_refiner)
+    check_onboarding(onboarding, H)
+    run_id = run_id or default_run_id(onboarding)
     p = plan(dataset_dir, setting, detections, dataset_name, depth=H > 0)
     check_out(out_dir)
-    prepare(model, dataset_dir, p, template_poses, template_level, pose_distribution, attach=H > 0)
+    prepare(model, dataset_dir, p, template_poses, template_level, pose_distribution, attach=H > 0,
+            onboarding=onboarding)
     run_images(model, p, range(len(p["images"])), out_dir, H, refine_masks, depth_refiner, vis_every)
     return write_csvs(model, p["name"], out_dir, run_id, H, refine_masks, depth_refiner)
 
@@ -687,6 +735,9 @@ def parser():
                          "(..._teaserpp.csv, no masks)")
     ap.add_argument("--vis-every", type=int, default=0, metavar="N",
                     help="write the retrieval panels of every N-th image to <out>/retrieved_sample_<i>.png (0: none)")
+    ap.add_argument("--onboarding", choices=("models", "static"), default="models",
+                    help="build the templates from the CAD models (models/) or, for objects without them, from the "
+                         "onboarding_static/ frames (model-free; no --refine-depth; run id bop_run_static)")
     ap.add_argument("--evaluate", action="store_true", help="score the csv (both, coarse first, when refining) with bop_eval")
     ap.add_argument("--device", default="cuda")
     return ap
@@ -701,6 +752,8 @@ def main(argv=None):
     if a.template_poses is not None and (a.template_level is not None or a.pose_distribution is not None):
         parser().error("--template-level and --pose-distribution choose generated template poses; "
                        "they do not go with --template-poses")
+    if a.onboarding == "static" and a.refine_depth:
+        parser().error(STATIC_NO_DEPTH)
     a.template_level = 1 if a.template_level is None else a.template_level
     a.pose_distribution = a.pose_distribution or "all"
     if int(os.environ.get("WORLD_SIZE", "1")) > 1:
@@ -708,7 +761,7 @@ def main(argv=None):
     model = build_model(a.device, a.out, checkpoint=a.checkpoint)
     csvs = run(model, a.dataset_dir, a.out, a.setting, a.detections, a.template_poses, refine_hypotheses=a.refine_depth,
                refine_masks=a.refine_masks, depth_refiner=a.depth_refiner, vis_every=a.vis_every,
-               template_level=a.template_level, pose_distribution=a.pose_distribution)
+               template_level=a.template_level, pose_distribution=a.pose_distribution, onboarding=a.onboarding)
     report(a, csvs, a.device)
 
 
@@ -737,7 +790,8 @@ def main_ranks(a):
             model = build_model(device, a.out, checkpoint=a.checkpoint)
             H = check_refine(model, a.refine_depth, a.refine_masks, a.depth_refiner)
             p = plan(a.dataset_dir, a.setting, a.detections, depth=H > 0)
-            prepare(model, a.dataset_dir, p, a.template_poses, a.template_level, a.pose_distribution, attach=H > 0)
+            prepare(model, a.dataset_dir, p, a.template_poses, a.template_level, a.pose_distribution, attach=H > 0,
+                    onboarding=a.onboarding)
             counts = [len(p["detections"][_key(s, im)]) for s, im in p["images"]]
             share = shard_images(counts, ranks.world_size)[ranks.rank]
             run_images(model, p, share, a.out, H, a.refine_masks, a.depth_refiner, a.vis_every)
@@ -745,7 +799,7 @@ def main_ranks(a):
 
         model, name, H = ranks.step(work)
         ranks.step(lambda: ranks.rank == 0 and report(
-            a, write_csvs(model, name, a.out, "bop_run", H, a.refine_masks, a.depth_refiner), device))
+            a, write_csvs(model, name, a.out, default_run_id(a.onboarding), H, a.refine_masks, a.depth_refiner), device))
     finally:
         ranks.close()
 

@@ -311,6 +311,31 @@ int gp_render_depth(int n_views, int height, int width, int num_vertices, const 
                     const int32_t* faces, const float* poses, const float* K, float z_near, void* workspace, float* depth,
                     int64_t* boxes, void* stream);
 
+/* --- row f16: onboarding from real frames with known poses (BOP onboarding_static).  The full contract is the header
+ * comment of gigapose_b200/csrc/onboard.cu.  Pixel centres are at integer coordinates, as gp_render_templates projects
+ * with K: pixel (column c, row r) is centred at (c, r).  virtual_to_source is HOST f64 [n,3,3] (row-major), the map
+ * H^-1 = K_f R_v^T K_t^-1 from a virtual pixel centre to frame pixel coordinates; a virtual pixel samples the frame at
+ * (x, y) = (s0 / s2, s1 / s2), s = H^-1 (c, r, 1)^T, and lies outside it when s2 <= 0 or the nearest pixel
+ * (rint(x), rint(y)) is outside [0, W) x [0, H).  Needs no handle. ----------------------------------------------------- */
+#define GP_RECENTRE_MAX_SIDE 16384   /* largest side, px, of a frame's box-scan region on the virtual grid */
+/* Boxes of the re-centred masks: masks u8 [n,H,W] (non-zero = object), src_boxes HOST i64 [n,4] xyxy (exclusive max)
+ * holding every non-zero pixel of each mask (x2 <= x1 for an empty mask).  out_boxes i64 [n,4] (device) gets, per
+ * frame, the xyxy box (exclusive max) of the virtual pixels whose nearest frame pixel is a mask pixel, on the
+ * unbounded virtual grid (coordinates may be negative or beyond any image size); (0, 0, 0, 0) when there is none.
+ * The scan region is the source box widened by 1 px and mapped through H; a frame whose region has a side over
+ * GP_RECENTRE_MAX_SIDE, or reaches the virtual camera's horizon, is refused with GP_ERR_INVALID naming the frame. */
+int gp_recentre_boxes(int n, int height, int width, const uint8_t* masks, const double* virtual_to_source,
+                      const int64_t* src_boxes, int64_t* out_boxes, void* stream);
+/* The 224 crops of the re-centred frames, straight from images u8 [n,H,W,3] (HWC) and masks u8 [n,H,W]: output pixel
+ * -> virtual pixel with gp_crop_resize_pad's index arithmetic for boxes i64 [n,4] (device, e.g. gp_recentre_boxes'
+ * output, non-empty; the box is never clipped), virtual pixel -> frame through virtual_to_source in fp64, RGB sampled
+ * bilinearly (indices clamped to the frame) and the mask by nearest, then rgb / 255, x mask and the CLIP mean / std as
+ * gp_crop_resize_pad_rle; 0 with mask 0 outside the frame.  Outputs out_images f32 [n,3,T,T], out_mask f32 [n,T,T] and
+ * out_M f32 [n,3,3], gp_crop_resize_pad's M for the box. */
+int gp_recentre_crop(int n, int height, int width, int target_size, const uint8_t* images, const uint8_t* masks,
+                     const double* virtual_to_source, const int64_t* boxes, float* out_images, float* out_mask,
+                     float* out_M, void* stream);
+
 /* --- row f7: BOP 2019 pose errors (the BOP toolkit's VSD / MSSD / MSPD that eval_bop19_pose.py computes for the
  * reference, src/scripts/eval_bop.py:16-38).  The full contract, with the fp32 operation order, is the header comment
  * of gigapose_b200/csrc/bop_eval.cu.  Needs no handle. -------------------------------------------------------------- */

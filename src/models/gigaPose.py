@@ -38,6 +38,14 @@ class _HostResult:
 RENDERS_NOT_KEPT = "renders not kept"      # GigaPose.template_views entry of a bank built by onboard_templates
 
 
+class CropViews:
+    """GigaPose.template_views entry of a bank built by onboard_images: `views(o, ids)` returns the template crops
+    (rgb [n,3,224,224], mask [n,224,224]) themselves rather than renders to crop."""
+
+    def __init__(self, views):
+        self.views = views
+
+
 def object_indices(infos, num_objects: int) -> np.ndarray:
     """0-based object indices from the `label` column (1-based ids as strings, gigaPose.py:514-520).  The reference
     indexes `template_data.ae_features[label - 1]`: label 0 silently wraps to the last object and label > O raises;
@@ -137,8 +145,10 @@ class GigaPose(LightningModule):
         self.use_cuda_graph = bool(kwargs.get("cuda_graph", False))
         self._graphs = {}
         # row f14: how `template_crops` gets each dataset's template crops back: a view renderer after onboard_meshes,
-        # RENDERS_NOT_KEPT after onboard_templates, no entry after set_template_data (read from template_datasets)
+        # a CropViews after onboard_images, RENDERS_NOT_KEPT after onboard_templates, no entry after set_template_data
+        # (read from template_datasets)
         self.template_views = {}
+        self.onboarding_views = {}           # row f16: frames chosen per template view by onboard_images
 
     # ------------------------------------------------------------------ out of scope: training
     def training_step(self, *a, **k):
@@ -244,11 +254,68 @@ class GigaPose(LightningModule):
 
         return self._onboard(dataset_name, n_obj, poses.shape[1], lambda o: views(o, slice(None)), K, poses, views)
 
+    @torch.no_grad()
+    def onboard_images(self, dataset_name, frames, template_poses):
+        """Row f16: onboarding from real frames with known poses, for objects without a CAD model (BOP's
+        onboarding_static sequences).  frames: one entry per object (label 1 first), each a
+        `gigapose_b200.onboarding.Frames` or a dict(images, masks, K [n,3,3], poses [n,4,4] object -> camera) with the
+        images as paths or u8 [H,W,3] and the masks as paths or [H,W] (non-zero = object); template_poses [T,4,4] the
+        viewpoints to cover.  For every template viewpoint the frame seen from the nearest direction is chosen
+        (`onboarding.select_frames`), re-centred on the object origin by a virtual camera with the template
+        intrinsics (`onboarding.recentre`) and cropped on the GPU (gp_recentre_boxes, gp_recentre_crop); the crops go
+        through the encoders into the bank as `onboard_templates`' do, with K = `render.TEMPLATE_K` and the virtual
+        poses.  `onboarding_views[dataset_name]` keeps the chosen frame ids and the angular gaps (degrees) per
+        object."""
+        import concurrent.futures
+
+        from gigapose_b200 import onboarding
+        from gigapose_b200.render import TEMPLATE_K
+        objs = [f if isinstance(f, onboarding.Frames) else onboarding.Frames(f["images"], f["masks"], f["K"], f["poses"])
+                for f in frames]
+        tpl = np.asarray(template_poses.cpu() if torch.is_tensor(template_poses) else template_poses, np.float64)
+        tpl = tpl.reshape(-1, 4, 4)
+        n_obj, T = len(objs), tpl.shape[0]
+        pool = concurrent.futures.ThreadPoolExecutor(onboarding.DECODE_THREADS)
+        chosen, poses = [], torch.empty(n_obj, T, 4, 4)
+        try:
+            def crops(o):
+                ids, gaps = onboarding.select_frames(objs[o], tpl, pool)
+                r = onboarding.recentre_frames(objs[o], ids, self.device, pool)
+                poses[o] = torch.as_tensor(r["poses"], dtype=torch.float32)
+                chosen.append((ids, gaps))
+                logger.info(f"{dataset_name} object {o + 1}: {len(np.unique(ids))} of {len(objs[o])} frames for {T} "
+                            f"views, largest gap {gaps.max():.1f} deg")
+                return r["images"], r["mask"], r["M"]
+
+            def views(o, ids):
+                r = onboarding.recentre_frames(objs[o], np.asarray(chosen[o][0])[np.asarray(ids)], self.device)
+                return r["images"].contiguous(), r["mask"].contiguous()
+
+            eng = self._onboard_crops(dataset_name, n_obj, T, crops, TEMPLATE_K, poses, CropViews(views))
+        finally:
+            pool.shutdown(wait=True)
+        self.onboarding_views[dataset_name] = dict(frame_ids=[c[0] for c in chosen], gap_deg=[c[1] for c in chosen])
+        logger.info(f"{dataset_name}: largest angular gap to a template view {max(c[1].max() for c in chosen):.1f} deg")
+        return eng
+
     def _onboard(self, dataset_name, n_obj, T, produce, K, poses, views):
-        """The body of both onboarding entry points: `produce(o)` -> (rgba [T,4,H,W] f32 on the device, boxes [T,4]);
-        `views(o, ids)` the same for the views `ids` only, kept for `template_crops` (or RENDERS_NOT_KEPT)."""
-        from gigapose_b200.engine import Engine
+        """The body of the render-based onboarding entry points: `produce(o)` -> (rgba [T,4,H,W] f32 on the device,
+        boxes [T,4]) cropped by `crop_resize_pad`; `views(o, ids)` the same for the views `ids` only, kept for
+        `template_crops` (or RENDERS_NOT_KEPT)."""
         from gigapose_b200.preprocess import CLIP_MEAN, CLIP_STD, crop_resize_pad
+
+        def crops(o):
+            rgba, boxes = produce(o)
+            crop = crop_resize_pad(torch.as_tensor(boxes), rgba, 224,
+                                   mean=CLIP_MEAN + (0.0,), std=CLIP_STD + (1.0,))      # alpha channel passes through
+            return crop["images"][:, :3], crop["images"][:, 3], crop["M"]
+
+        return self._onboard_crops(dataset_name, n_obj, T, crops, K, poses, views)
+
+    def _onboard_crops(self, dataset_name, n_obj, T, crops, K, poses, views):
+        """The body of every onboarding entry point: `crops(o)` -> (rgb [T,3,224,224] normalised, mask [T,224,224],
+        M [T,3,3]) on the device, streamed through both encoders into a new bank with K and poses."""
+        from gigapose_b200.engine import Engine
         device = self.device
         metric = self.testing_metric
         eng = Engine(n_obj, T, self.max_dets_per_call, device=device, k=metric.k, sim_threshold=metric.sim_threshold,
@@ -258,11 +325,9 @@ class GigaPose(LightningModule):
         builder = _BankBuilder(self, eng)
         Ms = []
         for o in range(n_obj):
-            rgba, boxes = produce(o)
-            crop = crop_resize_pad(torch.as_tensor(boxes), rgba, 224,
-                                   mean=CLIP_MEAN + (0.0,), std=CLIP_STD + (1.0,))      # alpha channel passes through
-            builder.add(o, crop["images"][:, :3], crop["images"][:, 3])
-            Ms.append(crop["M"])
+            rgb, mask, M = crops(o)
+            builder.add(o, rgb, mask)
+            Ms.append(M)
         builder.flush()
         K = torch.as_tensor(K, dtype=torch.float32, device=device)
         K = K.expand(n_obj, 3, 3).contiguous() if K.dim() == 2 else K
@@ -285,8 +350,8 @@ class GigaPose(LightningModule):
     def template_crops(self, dataset_name, obj, ids):
         """The normalised template crops f32 [n,3,224,224] and masks f32 [n,224,224] of views `ids` of object index
         `obj` (0-based) as the bank was built from them: read from `template_datasets` after `set_template_data`, and
-        re-rendered and re-cropped (the same `crop_resize_pad`) after `onboard_meshes`.  After `onboard_templates` the
-        caller's renders are not kept, so there is nothing to read them from: that raises ValueError."""
+        re-rendered and re-cropped (the same `crop_resize_pad`) after `onboard_meshes`, and re-decoded and re-centred
+        after `onboard_images`.  After `onboard_templates` the caller's renders are not kept, so there is nothing to read them from: that raises ValueError."""
         from gigapose_b200.preprocess import CLIP_MEAN, CLIP_STD, crop_resize_pad
         ids = torch.as_tensor(np.asarray(ids, np.int64))
         views = self.template_views.get(dataset_name)
@@ -296,6 +361,8 @@ class GigaPose(LightningModule):
         if views is None:
             data = self.template_datasets[dataset_name][obj]
             return data.rgb[ids].to(self.device).float(), data.mask[ids].to(self.device).float()
+        if isinstance(views, CropViews):
+            return views.views(obj, ids)
         rgba, boxes = views(obj, ids)
         crop = crop_resize_pad(torch.as_tensor(boxes), rgba, 224, mean=CLIP_MEAN + (0.0,), std=CLIP_STD + (1.0,))
         return crop["images"][:, :3].contiguous(), crop["images"][:, 3].contiguous()
