@@ -27,6 +27,7 @@ BOP_LABEL_FP, BOP_LABEL_TP, BOP_LABEL_IGNORED = 0, 1, 2          # GP_BOP_LABEL_
 BOP_ADD_CHUNK = 1024           # GP_BOP_ADD_CHUNK
 VIS_CROP = 224                 # GP_VIS_CROP
 VIS_MAX_SIDE = 16384           # GP_VIS_MAX_SIDE
+TSDF_MAX_VOXELS = 1 << 27      # GP_TSDF_MAX_VOXELS
 
 
 class GpConfig(C.Structure):
@@ -181,7 +182,14 @@ SYMBOLS = {
                                     C.POINTER(C.c_int64), C.c_void_p, C.c_void_p]),
     "gp_recentre_crop": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.POINTER(C.c_double),
                                    C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
-    "gp_bop_vsd": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p,
+    "gp_tsdf_fuse": (C.c_int, [C.c_int, C.c_int, C.c_int, C.POINTER(C.c_float), C.c_float, C.c_float, C.c_int,
+                               C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.POINTER(C.c_float), C.POINTER(C.c_float),
+                               C.c_void_p, C.c_void_p]),
+    "gp_tsdf_extract_query_sizes": (C.c_int, [C.c_int, C.c_int, C.c_int, C.POINTER(C.c_size_t)]),
+    "gp_tsdf_extract_count": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "gp_tsdf_extract_emit": (C.c_int, [C.c_int, C.c_int, C.c_int, C.POINTER(C.c_float), C.c_float, C.c_void_p,
+                                       C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "gp_bop_vsd":(C.c_int, [C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p,
                              C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_float,
                              C.c_int, C.POINTER(C.c_float), C.c_void_p, C.c_void_p, C.c_void_p]),
     "gp_bop_mssd_mspd": (C.c_int, [C.c_int, C.c_int, C.c_void_p, C.POINTER(C.c_int32), C.c_void_p, C.POINTER(C.c_int32),

@@ -26,7 +26,8 @@ Row f13, `--depth-refiner teaserpp` with `--refine-depth H`: the hypotheses go t
     python -m gigapose_b200.bop_run --dataset-dir D --checkpoint gigaPose_v1.ckpt
         [--template-poses P.npy | [--template-level 0|1|2] [--pose-distribution all|upper]]
         [--setting localization|detection] [--detections FILE] [--out DIR]
-        [--refine-depth H [--refine-masks | --depth-refiner teaserpp]] [--onboarding models|static] [--evaluate]
+        [--refine-depth H [--refine-masks | --depth-refiner teaserpp]] [--onboarding models|static [--reconstruct]]
+        [--evaluate]
 
 Row f15: without --template-poses the templates are the reference's test templates, generated
 (`template_poses.template_poses`, level 1 and all views by default).
@@ -34,8 +35,12 @@ Row f15: without --template-poses the templates are the reference's test templat
 Row f16, `--onboarding static`: objects without CAD models.  The templates are built from the dataset's
 onboarding_static/ frames (`onboard_static`, `GigaPose.onboard_images`) for the same template viewpoints; models/ is
 not read, except models_info.json when it exists (to check the object ids) and by --evaluate, whose BOP metrics need
-the models.  The depth refiners render the CAD model, so --refine-depth is refused; the default run id is
-`bop_run_static`.  Under `torchrun --nproc-per-node N -m
+the models.  The depth refiners render the CAD model, so --refine-depth is refused unless --reconstruct builds one;
+the default run id is `bop_run_static`.
+
+Row f17, `--onboarding static --refine-depth H --reconstruct`: every object is reconstructed from its onboarding depth
+images (`reconstruct.reconstruct`), written to <out>/reconstructed/obj_{id:06d}.ply and attached for the depth
+refiners, which then run as with CAD models.  Under `torchrun --nproc-per-node N -m
 gigapose_b200.bop_run ...` each rank runs its share of the images on its own GPU (`main_ranks`).
 """
 from __future__ import annotations
@@ -355,15 +360,15 @@ def onboard(model, dataset_dir, template_poses, dataset_name=None, meshes=None):
     return model.onboard_meshes(name, meshes, torch.as_tensor(poses, dtype=torch.float32))
 
 
-def onboard_static(model, dataset_dir, template_poses, dataset_name=None):
-    """`GigaPose.onboard_images` on the dataset's onboarding_static/ frames (`onboarding.read_onboarding_static`) for
-    the [T,4,4] template poses (an .npy path or an array)."""
+def onboard_static(model, dataset_dir, template_poses, dataset_name=None, frames=None):
+    """`GigaPose.onboard_images` on the dataset's onboarding_static/ frames (`onboarding.read_onboarding_static`,
+    unless the caller already holds them) for the [T,4,4] template poses (an .npy path or an array)."""
     from .onboarding import read_onboarding_static
     name = dataset_name or os.path.basename(os.path.normpath(dataset_dir))
     poses = np.load(template_poses) if isinstance(template_poses, (str, os.PathLike)) else np.asarray(template_poses)
     if poses.ndim != 3 or poses.shape[1:] != (4, 4):
         raise BopRunError(f"template poses must be [T,4,4], got {poses.shape}")
-    frames = read_onboarding_static(dataset_dir)
+    frames = read_onboarding_static(dataset_dir) if frames is None else frames
     return model.onboard_images(name, [frames[o] for o in sorted(frames)], poses)
 
 
@@ -537,30 +542,62 @@ def check_out(out_dir):
             raise BopRunError(f"{d} already holds prediction files; use an empty --out")
 
 
-def check_onboarding(onboarding, H):
+def check_onboarding(onboarding, H, reconstruct=False):
     if onboarding not in ("models", "static"):
         raise BopRunError(f"onboarding must be 'models' or 'static', got {onboarding!r}")
-    if onboarding == "static" and H:
+    if reconstruct and onboarding != "static":
+        raise BopRunError(RECONSTRUCT_NEEDS_STATIC)
+    if reconstruct and not H:
+        raise BopRunError(RECONSTRUCT_NEEDS_DEPTH)
+    if onboarding == "static" and H and not reconstruct:
         raise BopRunError(STATIC_NO_DEPTH)
 
 
 STATIC_NO_DEPTH = ("--onboarding static takes no --refine-depth: the depth refiners render the CAD model, which "
                    "model-free onboarding does not read")
+RECONSTRUCT_NEEDS_STATIC = "--reconstruct needs --onboarding static: it builds the meshes of model-free objects"
+RECONSTRUCT_NEEDS_DEPTH = "--reconstruct needs --refine-depth H: only the depth refiners use the reconstructed meshes"
+
+
+def reconstruct_meshes(frames, out_dir=None):
+    """Row f17: `reconstruct.reconstruct` of every object of {obj_id: Frames} (with depth), in object order; with
+    `out_dir`, each mesh is also written to out_dir/reconstructed/obj_{id:06d}.ply."""
+    from .reconstruct import reconstruct
+    from .render import write_ply
+    meshes = []
+    for o in sorted(frames):
+        try:
+            meshes.append(reconstruct(frames[o]))
+        except Exception as e:
+            e.add_note(f"while reconstructing object {o}")
+            raise
+        if out_dir is not None:
+            os.makedirs(os.path.join(out_dir, "reconstructed"), exist_ok=True)
+            write_ply(os.path.join(out_dir, "reconstructed", f"obj_{o:06d}.ply"), meshes[-1])
+    return meshes
 
 
 def prepare(model, dataset_dir, p, template_poses=None, template_level=1, pose_distribution="all", attach=False,
-            onboarding="models"):
+            onboarding="models", mesh_dir=None):
     """Onboards the plan's dataset unless the model already holds it, from `template_poses` or, when that is None,
     from the generated `template_poses.template_poses(template_level, pose_distribution)`; from the CAD models, or
     with onboarding="static" from the onboarding_static/ frames (`onboard_static`).  With `attach` (depth
-    refinement), attaches its meshes too."""
+    refinement), attaches its meshes too: the CAD models, or with onboarding="static" the meshes reconstructed from
+    the onboarding depth (`reconstruct_meshes`, written under `mesh_dir` when it is given)."""
     name = p["name"]
     if onboarding == "static":
+        attach = attach and name not in getattr(model, "meshes", {})
+        frames = None
+        if attach or name not in model.engines:
+            from .onboarding import read_onboarding_static
+            frames = read_onboarding_static(dataset_dir, depth=attach)
         if name not in model.engines:
             if template_poses is None:
                 from .template_poses import template_poses as generate
                 template_poses = generate(template_level, pose_distribution)
-            onboard_static(model, dataset_dir, template_poses, name)
+            onboard_static(model, dataset_dir, template_poses, name, frames)
+        if attach:
+            model.attach_meshes(name, reconstruct_meshes(frames, mesh_dir))
         return
     attach = attach and name not in getattr(model, "meshes", {})
     meshes = read_meshes(dataset_dir, name) if attach or name not in model.engines else None
@@ -626,7 +663,7 @@ def default_run_id(onboarding="models"):
 @torch.no_grad()
 def run(model, dataset_dir, out_dir, setting="localization", detections=None, template_poses=None, run_id=None,
         dataset_name=None, refine_hypotheses=0, refine_masks=False, depth_refiner="icp", vis_every=0,
-        template_level=1, pose_distribution="all", onboarding="models"):
+        template_level=1, pose_distribution="all", onboarding="models", reconstruct=False):
     """Runs the test split: onboards the dataset unless the model already holds it, from `template_poses` ([T,4,4]
     array or .npy path) or, when that is None, from the generated icosphere poses of `template_level` and
     `pose_distribution` (`template_poses.template_poses`, the reference's test templates by default), then one
@@ -641,14 +678,15 @@ def run(model, dataset_dir, out_dir, setting="localization", detections=None, te
     out_dir/retrieved_sample_{i}.png, one row per rank and one column per kept detection, as the reference does.
     With onboarding="static" (row f16) the templates come from the onboarding_static/ frames instead of the CAD
     models (`onboard_static`), refinement is refused, and the default run_id is "bop_run_static" ("bop_run"
-    otherwise)."""
+    otherwise).  With onboarding="static" and `reconstruct` (row f17), refinement is allowed: each object's mesh is
+    reconstructed from its onboarding depth images, written to out_dir/reconstructed/obj_{id:06d}.ply and attached."""
     H = check_refine(model, refine_hypotheses, refine_masks, depth_refiner)
-    check_onboarding(onboarding, H)
+    check_onboarding(onboarding, H, reconstruct)
     run_id = run_id or default_run_id(onboarding)
     p = plan(dataset_dir, setting, detections, dataset_name, depth=H > 0)
     check_out(out_dir)
     prepare(model, dataset_dir, p, template_poses, template_level, pose_distribution, attach=H > 0,
-            onboarding=onboarding)
+            onboarding=onboarding, mesh_dir=out_dir)
     run_images(model, p, range(len(p["images"])), out_dir, H, refine_masks, depth_refiner, vis_every)
     return write_csvs(model, p["name"], out_dir, run_id, H, refine_masks, depth_refiner)
 
@@ -737,7 +775,11 @@ def parser():
                     help="write the retrieval panels of every N-th image to <out>/retrieved_sample_<i>.png (0: none)")
     ap.add_argument("--onboarding", choices=("models", "static"), default="models",
                     help="build the templates from the CAD models (models/) or, for objects without them, from the "
-                         "onboarding_static/ frames (model-free; no --refine-depth; run id bop_run_static)")
+                         "onboarding_static/ frames (model-free; --refine-depth only with --reconstruct; run id "
+                         "bop_run_static)")
+    ap.add_argument("--reconstruct", action="store_true",
+                    help="with --onboarding static and --refine-depth: reconstruct each object from its onboarding "
+                         "depth images (<out>/reconstructed/obj_<id>.ply) and refine against that mesh")
     ap.add_argument("--evaluate", action="store_true", help="score the csv (both, coarse first, when refining) with bop_eval")
     ap.add_argument("--device", default="cuda")
     return ap
@@ -752,7 +794,11 @@ def main(argv=None):
     if a.template_poses is not None and (a.template_level is not None or a.pose_distribution is not None):
         parser().error("--template-level and --pose-distribution choose generated template poses; "
                        "they do not go with --template-poses")
-    if a.onboarding == "static" and a.refine_depth:
+    if a.reconstruct and a.onboarding != "static":
+        parser().error(RECONSTRUCT_NEEDS_STATIC)
+    if a.reconstruct and not a.refine_depth:
+        parser().error(RECONSTRUCT_NEEDS_DEPTH)
+    if a.onboarding == "static" and a.refine_depth and not a.reconstruct:
         parser().error(STATIC_NO_DEPTH)
     a.template_level = 1 if a.template_level is None else a.template_level
     a.pose_distribution = a.pose_distribution or "all"
@@ -761,7 +807,8 @@ def main(argv=None):
     model = build_model(a.device, a.out, checkpoint=a.checkpoint)
     csvs = run(model, a.dataset_dir, a.out, a.setting, a.detections, a.template_poses, refine_hypotheses=a.refine_depth,
                refine_masks=a.refine_masks, depth_refiner=a.depth_refiner, vis_every=a.vis_every,
-               template_level=a.template_level, pose_distribution=a.pose_distribution, onboarding=a.onboarding)
+               template_level=a.template_level, pose_distribution=a.pose_distribution, onboarding=a.onboarding,
+               reconstruct=a.reconstruct)
     report(a, csvs, a.device)
 
 
@@ -777,8 +824,9 @@ def report(a, csvs, device):
 def main_ranks(a):
     """`main` under torchrun: every rank builds the model on cuda:LOCAL_RANK (or on --device when it names a device
     index, so that several ranks can share one GPU), onboards the dataset itself and runs its `shard_images` share of
-    the plan's images into the same --out; rank 0 checks --out first and writes the csv(s) and scores last.  A rank
-    that fails makes every rank exit with its error (`Ranks.step`)."""
+    the plan's images into the same --out; rank 0 checks --out first and writes the csv(s) and scores last (and, with
+    --reconstruct, the meshes, which every rank reconstructs alike: the kernels are deterministic).  A rank that
+    fails makes every rank exit with its error (`Ranks.step`)."""
     ranks = Ranks()
     try:
         device = torch.device(f"cuda:{os.environ.get('LOCAL_RANK', '0')}" if a.device == "cuda" else a.device)
@@ -791,7 +839,7 @@ def main_ranks(a):
             H = check_refine(model, a.refine_depth, a.refine_masks, a.depth_refiner)
             p = plan(a.dataset_dir, a.setting, a.detections, depth=H > 0)
             prepare(model, a.dataset_dir, p, a.template_poses, a.template_level, a.pose_distribution, attach=H > 0,
-                    onboarding=a.onboarding)
+                    onboarding=a.onboarding, mesh_dir=a.out if ranks.rank == 0 else None)
             counts = [len(p["detections"][_key(s, im)]) for s, im in p["images"]]
             share = shard_images(counts, ranks.world_size)[ranks.rank]
             run_images(model, p, share, a.out, H, a.refine_masks, a.depth_refiner, a.vis_every)

@@ -8,11 +8,12 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libgigapose_b200.so")
-SOURCES = ["runtime.cu", "api.cu", "sim_search.cu", "prep.cu", "ist_mlp.cu", "ransac_pose.cu", "vit_gemm.cu", "vit_ops.cu", "vit_attention_tc.cu", "vit_api.cu", "ist_trunk.cu", "preprocess.cu", "render.cu", "depth_icp.cu", "depth_score.cu", "bop_eval.cu", "depth_teaser.cu", "vis.cu", "onboard.cu"]
+SOURCES = ["runtime.cu", "api.cu", "sim_search.cu", "prep.cu", "ist_mlp.cu", "ransac_pose.cu", "vit_gemm.cu", "vit_ops.cu", "vit_attention_tc.cu", "vit_api.cu", "ist_trunk.cu", "preprocess.cu", "render.cu", "depth_icp.cu", "depth_score.cu", "bop_eval.cu", "depth_teaser.cu", "vis.cu", "onboard.cu", "reconstruct.cu"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
               "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr"]
 # sources whose contract states every floating-point operation rounds once (no multiply-add contraction)
-SOURCE_FLAGS = {"depth_teaser.cu": ["-fmad=false"], "onboard.cu": ["-fmad=false"]}
+SOURCE_FLAGS = {"depth_teaser.cu": ["-fmad=false"], "onboard.cu": ["-fmad=false"],
+                "reconstruct.cu": ["-fmad=false"]}
 
 
 def _nvcc() -> str:

@@ -171,11 +171,27 @@ def read_mask(x):
     return (a != 0).astype(np.uint8)
 
 
+def read_depth(x, depth_scale):
+    """Path (16-bit PNG) or array / tensor [H,W] -> f32 [H,W] in the unit of the poses: the raw values x depth_scale
+    in fp64, rounded once to f32 (`bop_eval.load_depth`'s rule); 0 = missing."""
+    if isinstance(x, (str, os.PathLike)):
+        from PIL import Image
+        with Image.open(x) as im:
+            a = np.asarray(im)
+    else:
+        a = x.cpu().numpy() if torch.is_tensor(x) else np.asarray(x)
+    if a.ndim != 2:
+        raise OnboardingError(f"an onboarding depth image must be [H,W], got shape {a.shape}")
+    return (a.astype(np.float64) * float(depth_scale)).astype(np.float32)
+
+
 class Frames:
     """One object's onboarding frames: images and masks (paths, or u8 arrays / tensors [H,W,3] and [H,W]), K [n,3,3]
-    and poses [n,4,4] object -> camera.  Masks are decoded once, when first asked for (`valid`, `load`)."""
+    and poses [n,4,4] object -> camera.  Masks are decoded once, when first asked for (`valid`, `load`).  Optional
+    depths (16-bit PNG paths or arrays [H,W]) with depth_scale (one value, or one per frame; default 1) hold the
+    depth images of row f17's reconstruction (`load_depth`)."""
 
-    def __init__(self, images, masks, K, poses):
+    def __init__(self, images, masks, K, poses, depths=None, depth_scale=None):
         self.images, self.masks = list(images), list(masks)
         n = len(self.images)
         self.K = np.asarray(K, np.float64).reshape(-1, 3, 3)
@@ -185,6 +201,13 @@ class Frames:
                                   f"{self.poses.shape[0]} poses: one of each per frame")
         if n == 0:
             raise OnboardingError("an object has no onboarding frames")
+        self.depths = None if depths is None else list(depths)
+        if self.depths is not None and len(self.depths) != n:
+            raise OnboardingError(f"{n} frames and {len(self.depths)} depth images: one per frame")
+        scale = np.broadcast_to(np.asarray(1.0 if depth_scale is None else depth_scale, np.float64), (n,)).copy()
+        if not np.all(np.isfinite(scale) & (scale > 0)):
+            raise OnboardingError("depth_scale must be positive and finite")
+        self.depth_scale = scale
         self.boxes = {}                                         # frame -> source mask box, once decoded
 
     def __len__(self):
@@ -202,6 +225,12 @@ class Frames:
             raise OnboardingError(f"frame {i}: image {rgb.shape[:2]} and mask {m.shape} differ in size"
                                   + (f" ({self.images[i]})" if isinstance(self.images[i], (str, os.PathLike)) else ""))
         return rgb, m
+
+    def load_depth(self, i):
+        """-> depth f32 [H,W] of frame i in the unit of the poses (0 = missing)."""
+        if self.depths is None:
+            raise OnboardingError("these frames carry no depth images")
+        return read_depth(self.depths[i], self.depth_scale[i])
 
 
 def select_frames(frames, template_poses, pool=None):
@@ -275,13 +304,14 @@ def _load_json(path):
         return json.load(f)
 
 
-def read_onboarding_static(dataset_dir):
+def read_onboarding_static(dataset_dir, depth=False):
     """The dataset's onboarding_static/ tree (the layout of the BOP 2024 H3 datasets: one directory per scene, e.g.
     obj_000001_up and obj_000001_down, each with rgb/{im:06d}.jpg (or .png), mask_visib/{im:06d}_000000.png,
     scene_gt.json and scene_camera.json, one object per scene) -> {obj_id: Frames} with the up and down scenes of each
     object together, in scene then image order.  Refuses, naming the file or scene: a scene whose scene_gt holds more
     than one object, a missing mask or image, object ids that are not 1 .. N, and, when models/models_info.json exists,
-    an id set that differs from it."""
+    an id set that differs from it.  With `depth` (row f17) the frames also carry depth/{im:06d}.png and the image's
+    `depth_scale` from scene_camera.json; a missing depth image or depth_scale is refused, naming it."""
     root = os.path.join(dataset_dir, "onboarding_static")
     if not os.path.isdir(root):
         raise OnboardingError(f"{root} not found: model-free onboarding reads the onboarding_static sequences")
@@ -298,7 +328,7 @@ def read_onboarding_static(dataset_dir):
             raise OnboardingError(f"{os.path.join(d, 'scene_gt.json')}: scene {sc} must show one object once per image, "
                                   f"found objects {sorted(ids)}")
         obj = ids.pop()
-        acc = per_obj.setdefault(obj, dict(images=[], masks=[], K=[], poses=[]))
+        acc = per_obj.setdefault(obj, dict(images=[], masks=[], K=[], poses=[], depths=[], depth_scale=[]))
         for im in sorted(int(k) for k in gt):
             e = gt[str(im)][0]
             if str(im) not in cam:
@@ -317,6 +347,14 @@ def read_onboarding_static(dataset_dir):
             acc["masks"].append(mask)
             acc["K"].append(np.asarray(cam[str(im)]["cam_K"], np.float64).reshape(3, 3))
             acc["poses"].append(pose)
+            if depth:
+                dpath = os.path.join(d, "depth", f"{im:06d}.png")
+                if not os.path.exists(dpath):
+                    raise OnboardingError(f"{dpath} not found: reconstruction fuses the onboarding depth images")
+                if "depth_scale" not in cam[str(im)]:
+                    raise OnboardingError(f"{os.path.join(d, 'scene_camera.json')}: image {im} has no depth_scale")
+                acc["depths"].append(dpath)
+                acc["depth_scale"].append(float(cam[str(im)]["depth_scale"]))
     found = sorted(per_obj)
     if found != list(range(1, len(found) + 1)):
         raise OnboardingError(f"{root}: object ids {found} are not 1 .. {len(found)}: labels index the template bank")
@@ -325,5 +363,7 @@ def read_onboarding_static(dataset_dir):
         listed = sorted(int(k) for k in _load_json(info))
         if listed != found:
             raise OnboardingError(f"{info} lists objects {listed} but {root} has objects {found}")
-    return {o: Frames(v["images"], v["masks"], np.stack(v["K"]), np.stack(v["poses"])) for o, v in sorted(per_obj.items())}
+    return {o: Frames(v["images"], v["masks"], np.stack(v["K"]), np.stack(v["poses"]),
+                      v["depths"] if depth else None, v["depth_scale"] if depth else None)
+            for o, v in sorted(per_obj.items())}
 

@@ -162,6 +162,26 @@ def read_ply(path):
     return dict(vertices=V, faces=faces, vertex_color=color, face_uv=uv if texture is not None else None, texture=texture)
 
 
+def write_ply(path, mesh):
+    """Writes the vertices f32 [V,3] and faces i32 [F,3] of a mesh dict as binary little-endian PLY (x y z floats,
+    uchar-counted int vertex_indices); `read_ply` reads them back bit for bit.  Colours and textures are not written."""
+    V = np.ascontiguousarray(np.asarray(mesh["vertices"], np.float32).reshape(-1, 3))
+    F = np.asarray(mesh["faces"]).reshape(-1, 3)
+    if not np.isfinite(V).all():
+        raise PlyError("non-finite vertex coordinates")
+    if F.size and (F.min() < 0 or F.max() >= len(V)):
+        raise PlyError(f"face indices outside [0, {len(V)})")
+    rows = np.empty(len(F), np.dtype([("n", "u1"), ("i", "<i4", (3,))]))
+    rows["n"] = 3
+    rows["i"] = F
+    header = (f"ply\nformat binary_little_endian 1.0\nelement vertex {len(V)}\nproperty float x\nproperty float y\n"
+              f"property float z\nelement face {len(F)}\nproperty list uchar int vertex_indices\nend_header\n")
+    with open(path, "wb") as f:
+        f.write(header.encode("ascii"))
+        f.write(V.astype("<f4").tobytes())
+        f.write(rows.tobytes())
+
+
 def _device_mesh(mesh, device):
     """Mesh dict -> contiguous device tensors; a texture takes precedence over vertex colours."""
     def t(x, dtype):

@@ -336,6 +336,27 @@ int gp_recentre_crop(int n, int height, int width, int target_size, const uint8_
                      const double* virtual_to_source, const int64_t* boxes, float* out_images, float* out_mask,
                      float* out_M, void* stream);
 
+/* --- row f17: reconstruction from onboarding RGB-D frames (TSDF fusion, marching tetrahedra).  The full contract,
+ * with the fp32 operation order, is the header comment of gigapose_b200/csrc/reconstruct.cu.  The grid is f32
+ * [nz,ny,nx,2] of (tsdf, weight) pairs, voxel (x, y, z) centred at origin + ((x, y, z) + 0.5) * voxel in the object
+ * frame (origin HOST f32 [3]).  Needs no handle. ------------------------------------------------------------------- */
+#define GP_TSDF_MAX_VOXELS 134217728   /* 2^27 voxels: at most 12 triangles per cube keep counts within int32 */
+/* Fuses n_frames frames into `grid` (zeroed by the caller before its first frame), in order: depth f32 [n,H,W] in the
+ * unit of the poses (0 = missing), masks u8 [n,H,W] (non-zero = object), K and poses HOST f32 [n,3,3] (last row
+ * 0 0 1) and [n,4,4] object -> camera; trunc = mu > 0 in the same unit. */
+int gp_tsdf_fuse(int nx, int ny, int nz, const float* origin, float voxel, float trunc, int n_frames, int height,
+                 int width, const float* depth, const uint8_t* masks, const float* K, const float* poses, float* grid,
+                 void* stream);
+/* Workspace bytes of the extraction of an nx x ny x nz grid (every side >= 2). */
+int gp_tsdf_extract_query_sizes(int nx, int ny, int nz, size_t* workspace_bytes);
+/* Count pass: marks the crossed edges, scans the vertex and face counts in the workspace and writes counts i64 [2]
+ * (device) = (vertices, faces). */
+int gp_tsdf_extract_count(int nx, int ny, int nz, const float* grid, void* workspace, int64_t* counts, void* stream);
+/* Emit pass, after gp_tsdf_extract_count on the same grid and workspace: vertices f32 [V,3] in the object frame and
+ * faces i32 [F,3] (V, F >= 1: the counts it wrote), both in row-major voxel order. */
+int gp_tsdf_extract_emit(int nx, int ny, int nz, const float* origin, float voxel, const float* grid,
+                         const void* workspace, float* vertices, int32_t* faces, void* stream);
+
 /* --- row f7: BOP 2019 pose errors (the BOP toolkit's VSD / MSSD / MSPD that eval_bop19_pose.py computes for the
  * reference, src/scripts/eval_bop.py:16-38).  The full contract, with the fp32 operation order, is the header comment
  * of gigapose_b200/csrc/bop_eval.cu.  Needs no handle. -------------------------------------------------------------- */
