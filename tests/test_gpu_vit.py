@@ -1,6 +1,9 @@
 """-m gpu parity of the native ViT forward (row a1) against the fp32 CPU restatement (oracle/port.py::DinoV2Port,
 itself pinned by tests/golden/backbones.npz and cross-checked against transformers' Dinov2).  Tolerances are
-floating-point: the split-bf16 tensor-core GEMMs are fp32-faithful to ~1e-5 per layer."""
+floating-point: measured block by block against fp64 (tests/test_gpu_vit_fp64.py, H100 80GB HBM3 at 700 W), each ViT
+block is within 4.1e-6 of the magnitude sum of its output, the 24-block x_prenorm within 8.1e-4 of the last block's
+sum, and the unit-norm descriptors within 2.7e-6 absolute.  These weights have every LayerScale at 1, so the
+LayerScale wiring is checked there, not here."""
 import pytest
 import torch
 
