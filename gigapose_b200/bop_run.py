@@ -58,6 +58,7 @@ import numpy as np
 import torch
 
 from .bop_eval import load_cameras, load_depth
+from .teaser import REFINERS
 
 CAP_PER_TARGET = 16             # localization: detections kept per target (dataloader/test.py:110-114)
 CAP_PER_TARGET_ICBIN = 32
@@ -494,14 +495,12 @@ def refine_image(model, p, i, kept, depth, hypotheses, out_dir, masks=None, refi
     depth = torch.as_tensor(depth).to(device, non_blocking=True)
     K = torch.as_tensor(p["cameras"][s][im], dtype=torch.float64).float()
     extra = {} if masks is None else dict(masks=dict(counts=masks[0], offsets=masks[1]), mask_normals=True)
-    if refiner != "icp":
-        extra["refiner"] = refiner
     refined = model.refine_depth(p["name"], kept, depth[None], frame_idx=np.zeros(n, np.int64), hypotheses=hypotheses,
-                                 K=K, rank=True, **extra)
+                                 K=K, rank=True, refiner=refiner, **extra)
     rows = torch.arange(n, device=device)
     poses = refined.pred_poses[rows, refined.best_hypothesis]
     scores = kept.scores[rows, refined.best_hypothesis]
-    status_key = "icp_status" if refiner == "icp" else "teaser_status"
+    status_key = REFINERS[refiner].outputs[0]
     status = getattr(refined, status_key)[rows, refined.best_hypothesis]
     stop.record()
     stop.synchronize()
@@ -526,10 +525,10 @@ def check_refine(model, refine_hypotheses, refine_masks, depth_refiner):
         raise BopRunError(f"refine_hypotheses {H} outside [0, {model.testing_metric.k}]")
     if refine_masks and not H:
         raise BopRunError("refine_masks needs refine_hypotheses >= 1")
-    if depth_refiner not in ("icp", "teaserpp"):
-        raise BopRunError(f"depth_refiner must be 'icp' or 'teaserpp', got {depth_refiner!r}")
-    if depth_refiner == "teaserpp" and refine_masks:
-        raise BopRunError("the teaserpp depth refiner takes no masks (refine_masks)")
+    if depth_refiner not in REFINERS:
+        raise BopRunError(f"depth_refiner must be {' or '.join(map(repr, REFINERS))}, got {depth_refiner!r}")
+    if refine_masks and not REFINERS[depth_refiner].masks:
+        raise BopRunError(f"the {depth_refiner} depth refiner takes no masks (refine_masks)")
     return H
 
 
@@ -650,7 +649,7 @@ def write_csvs(model, name, out_dir, run_id="bop_run", H=0, refine_masks=False, 
     coarse = os.path.join(pred_dir, f"{stem}.csv")
     if not H:
         return coarse
-    suffix = "_teaserpp" if depth_refiner == "teaserpp" else "_icp_masked" if refine_masks else "_icp"
+    suffix = f"_{depth_refiner}_masked" if refine_masks else f"_{depth_refiner}"
     save_predictions_from_batched_predictions(ref_dir, dataset_name=name, model_name=model.model_name,
                                               run_id=f"{run_id}{suffix}", is_refined=True)
     return coarse, os.path.join(ref_dir, f"{stem}{suffix}.csv")
@@ -768,7 +767,7 @@ def parser():
     ap.add_argument("--refine-masks", action="store_true",
                     help="with --refine-depth: refine each instance with its own CNOS mask, target normals smoothed "
                          "within it (writes ..._icp_masked.csv)")
-    ap.add_argument("--depth-refiner", choices=("icp", "teaserpp"), default="icp",
+    ap.add_argument("--depth-refiner", choices=tuple(REFINERS), default="icp",
                     help="with --refine-depth: the point-to-plane ICP (..._icp.csv) or MegaPose's TEASER++ refiner "
                          "(..._teaserpp.csv, no masks)")
     ap.add_argument("--vis-every", type=int, default=0, metavar="N",
@@ -789,8 +788,8 @@ def main(argv=None):
     a = parser().parse_args(argv)
     if a.refine_masks and not a.refine_depth:
         parser().error("--refine-masks needs --refine-depth H")
-    if a.depth_refiner == "teaserpp" and a.refine_masks:
-        parser().error("--depth-refiner teaserpp takes no --refine-masks")
+    if a.refine_masks and not REFINERS[a.depth_refiner].masks:
+        parser().error(f"--depth-refiner {a.depth_refiner} takes no --refine-masks")
     if a.template_poses is not None and (a.template_level is not None or a.pose_distribution is not None):
         parser().error("--template-level and --pose-distribution choose generated template poses; "
                        "they do not go with --template-poses")

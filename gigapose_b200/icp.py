@@ -22,17 +22,37 @@ STATUS_NAMES = {_lib.ICP_OK: "ok", _lib.ICP_TOO_FEW_POINTS: "too few points", _l
                 _lib.ICP_LOST: "lost: no pairs, or fewer than 6 kept"}
 DEFAULTS = dict(unit_per_m=1000.0, min_points=1000, num_levels=4, max_iters=100, rejection_scale=2.5,
                 max_residual=0.01, min_step_rad=1e-6, min_step_m=1e-6)
-WORKSPACE_BYTES = 1 << 30          # renders + ICP scratch per chunk of hypotheses: ~20 MB per 640 x 480 hypothesis
+WORKSPACE_BYTES = 1 << 30          # renders + refiner scratch per chunk of hypotheses: ~20 MB per 640 x 480 hypothesis
+
+
+def _params(struct, debug_struct, defaults, what, debug, params):
+    """A refiner's params `struct` from `defaults` updated with `params`, and its debug member from `debug` (ints as
+    they are, tensors as device addresses); unknown names raise TypeError."""
+    unknown = set(params) - set(defaults)
+    if unknown:
+        raise TypeError(f"unknown {what} parameters {sorted(unknown)}")
+    out = struct(**dict(defaults, **params))
+    if debug:
+        out.debug = debug_struct(**{k: v if isinstance(v, int) else ptr(v) for k, v in debug.items()})
+    return out
 
 
 def make_params(debug=None, **params) -> GpIcpParams:
-    unknown = set(params) - set(DEFAULTS)
-    if unknown:
-        raise TypeError(f"unknown ICP parameters {sorted(unknown)}")
-    p = dict(DEFAULTS, **params)
-    out = GpIcpParams(**p)
-    if debug:
-        out.debug = GpIcpDebug(**{k: v if isinstance(v, int) else ptr(v) for k, v in debug.items()})
+    return _params(GpIcpParams, GpIcpDebug, DEFAULTS, "ICP", debug, params)
+
+
+def _outputs(n, device, dtype):
+    """A refiner's four per-hypothesis outputs: poses f32 [n,4,4], status i32 [n] and two [n] of `dtype`."""
+    return (torch.empty(n, 4, 4, device=device), torch.empty(n, dtype=torch.int32, device=device),
+            torch.empty(n, dtype=dtype, device=device), torch.empty(n, dtype=dtype, device=device))
+
+
+def _refine_call(entry, args, n, device, dtype, *workspaces):
+    """A refiner's entry point on n hypotheses: `args` (everything before its outputs), its `_outputs`, `workspaces`
+    and the current stream.  -> the outputs."""
+    out = _outputs(n, device, dtype)
+    check(entry(*args, *(t.data_ptr() for t in out), *(w.data_ptr() for w in workspaces),
+                torch.cuda.current_stream(device).cuda_stream))
     return out
 
 
@@ -85,17 +105,10 @@ def refine_rendered(depth, K, frame_idx, rendered, boxes, poses, masks, workspac
     """gp_icp_refine over n hypotheses whose scene is already in `workspace` -> poses, status, residual, fitness."""
     F, H, W = depth.shape
     n = poses.shape[0]
-    dev = poses.device
-    out = torch.empty(n, 4, 4, device=dev)
-    status = torch.empty(n, dtype=torch.int32, device=dev)
-    residual = torch.empty(n, device=dev)
-    fitness = torch.empty(n, device=dev)
     p = make_params(debug, **params)
-    check(_lib.load().gp_icp_refine(F, n, H, W, frame_idx.data_ptr(), ptr(masks), rendered.data_ptr(), boxes.data_ptr(),
-                                    poses.data_ptr(), K.data_ptr(), C.byref(p), out.data_ptr(), status.data_ptr(),
-                                    residual.data_ptr(), fitness.data_ptr(), workspace.data_ptr(),
-                                    torch.cuda.current_stream(dev).cuda_stream))
-    return out, status, residual, fitness
+    return _refine_call(_lib.load().gp_icp_refine, (F, n, H, W, frame_idx.data_ptr(), ptr(masks), rendered.data_ptr(),
+                                                    boxes.data_ptr(), poses.data_ptr(), K.data_ptr(), C.byref(p)),
+                        n, poses.device, torch.float32, workspace)
 
 
 def _inputs(what, meshes_dev, labels, poses, depth, K, frame_idx):
@@ -125,6 +138,26 @@ def _inputs(what, meshes_dev, labels, poses, depth, K, frame_idx):
     return poses, depth, K, labels, frame_idx
 
 
+def _chunk(n, per_hyp_bytes, H, W, group=1):
+    """Hypotheses per chunk: whole groups of `group` whose renders (52 B per pixel) and `per_hyp_bytes` of scratch
+    each fit WORKSPACE_BYTES, at least one group."""
+    return group * max(1, min(n // group, WORKSPACE_BYTES // (group * (per_hyp_bytes + 52 * H * W))))
+
+
+def _render_and_run(meshes_dev, labels, poses, K, frame_idx, H, W, upm, per_hyp_bytes, run, outputs, group=1):
+    """Renders the n hypotheses (`_inputs`' layout) chunk by chunk (`_chunk`), calls run(slice, rendered, boxes) on
+    each chunk and copies the per-hypothesis tensors it returns into the chunk's rows of `outputs`.  Every result
+    depends on its own hypothesis (or group) only, so the chunking changes no output.  -> `outputs`."""
+    n = poses.shape[0]
+    chunk = _chunk(n, per_hyp_bytes, H, W, group)
+    for s in range(0, n, chunk):
+        sl = slice(s, min(n, s + chunk))
+        rendered, boxes = render_hypotheses(meshes_dev, labels[sl], poses[sl], K, frame_idx[sl], H, W, upm)
+        for o, r in zip(outputs, run(sl, rendered, boxes)):
+            o[sl] = r
+    return outputs
+
+
 @torch.no_grad()
 def refine_icp(meshes_dev, labels, poses, depth, K, frame_idx, masks=None, **params):
     """Refines n hypotheses against the measured depth.
@@ -143,25 +176,18 @@ def refine_icp(meshes_dev, labels, poses, depth, K, frame_idx, masks=None, **par
     n = poses.shape[0]
     if masks is not None:
         masks = torch.as_tensor(masks).to(device).reshape(n, H, W).to(torch.uint8).contiguous()
-    out = poses.clone()
-    status = torch.empty(n, dtype=torch.int32, device=device)
-    residual = torch.empty(n, device=device)
-    fitness = torch.empty(n, device=device)
+    out = _outputs(n, device, torch.float32)
     if n == 0:
-        return out, status, residual, fitness
+        return out
     scene = workspace_bytes(F, 0, H, W)
     per_hyp = workspace_bytes(F, 1, H, W) - scene
-    chunk = max(1, min(n, WORKSPACE_BYTES // (per_hyp + 52 * H * W)))
-    ws = torch.empty(scene + chunk * per_hyp, dtype=torch.uint8, device=device)
+    ws = torch.empty(scene + _chunk(n, per_hyp, H, W) * per_hyp, dtype=torch.uint8, device=device)
     prepare_scene(depth, K, ws, upm)
     fi = frame_idx.to(device, torch.int32)
-    for s in range(0, n, chunk):
-        sl = slice(s, min(n, s + chunk))
-        rendered, boxes = render_hypotheses(meshes_dev, labels[sl], poses[sl], K, frame_idx[sl], H, W, upm)
-        o = refine_rendered(depth, K, fi[sl].contiguous(), rendered, boxes, poses[sl],
-                            None if masks is None else masks[sl], ws, **params)
-        out[sl], status[sl], residual[sl], fitness[sl] = o
-    return out, status, residual, fitness
+    return _render_and_run(meshes_dev, labels, poses, K, frame_idx, H, W, upm, per_hyp,
+                           lambda sl, rendered, boxes: refine_rendered(depth, K, fi[sl].contiguous(), rendered, boxes,
+                                                                       poses[sl], None if masks is None else masks[sl],
+                                                                       ws, **params), out)
 
 
 @torch.no_grad()
@@ -182,22 +208,22 @@ def score_hypotheses(meshes_dev, labels, poses, depth, K, frame_idx, n_hyp, tole
     n = poses.shape[0]
     if n % n_hyp:
         raise ValueError(f"{n} poses are not a whole number of groups of {n_hyp} hypotheses")
-    n_det = n // n_hyp
     if not torch.equal(frame_idx, frame_idx[::n_hyp].repeat_interleave(n_hyp)):
         raise ValueError("the hypotheses of a detection must share one frame")
     counts = torch.empty(n, 4, dtype=torch.int32, device=device)
     score = torch.empty(n, device=device)
-    best = torch.empty(n_det, dtype=torch.int32, device=device)
+    best = torch.empty(n // n_hyp, dtype=torch.int32, device=device)
     fi = frame_idx[::n_hyp].to(device, torch.int32)
-    chunk = max(1, min(n_det, WORKSPACE_BYTES // (52 * H * W * n_hyp)))      # detections per chunk, renders as above
-    for s in range(0, n_det, chunk):
-        e = min(n_det, s + chunk)
-        sl = slice(s * n_hyp, e * n_hyp)
-        rendered, boxes = render_hypotheses(meshes_dev, labels[sl], poses[sl], K, frame_idx[sl], H, W, unit_per_m)
-        check(_lib.load().gp_depth_score(F, e - s, n_hyp, H, W, fi[s:e].data_ptr(), depth.data_ptr(),
+
+    def run(sl, rendered, boxes):                                      # writes the chunk's rows in place
+        det = slice(sl.start // n_hyp, sl.stop // n_hyp)
+        check(_lib.load().gp_depth_score(F, det.stop - det.start, n_hyp, H, W, fi[det].data_ptr(), depth.data_ptr(),
                                          rendered.data_ptr(), boxes.data_ptr(), float(tolerance_m) * float(unit_per_m),
-                                         counts[sl].data_ptr(), score[sl].data_ptr(), best[s:e].data_ptr(),
+                                         counts[sl].data_ptr(), score[sl].data_ptr(), best[det].data_ptr(),
                                          torch.cuda.current_stream(device).cuda_stream))
+        return ()
+
+    _render_and_run(meshes_dev, labels, poses, K, frame_idx, H, W, unit_per_m, 0, run, (), group=n_hyp)
     return counts, score, best
 
 
@@ -313,19 +339,11 @@ def refine_rendered_masked(ms, scene_ws, box_pixels, depth, K, det_idx, rendered
     """gp_icp_refine_masked over n hypotheses against a prepared masked scene -> poses, status, residual, fitness."""
     F, H, W = depth.shape
     n = poses.shape[0]
-    dev = poses.device
-    out = torch.empty(n, 4, 4, device=dev)
-    status = torch.empty(n, dtype=torch.int32, device=dev)
-    residual = torch.empty(n, device=dev)
-    fitness = torch.empty(n, device=dev)
-    scratch = torch.empty(max(n * box_pixels * 12, 1), dtype=torch.uint8, device=dev)
+    scratch = torch.empty(max(n * box_pixels * 12, 1), dtype=torch.uint8, device=poses.device)
     p = make_params(debug, **params)
-    check(_lib.load().gp_icp_refine_masked(F, H, W, C.byref(ms.c), n, det_idx.data_ptr(), rendered.data_ptr(),
-                                           boxes.data_ptr(), poses.data_ptr(), K.data_ptr(), C.byref(p), out.data_ptr(),
-                                           status.data_ptr(), residual.data_ptr(), fitness.data_ptr(),
-                                           scene_ws.data_ptr(), scratch.data_ptr(),
-                                           torch.cuda.current_stream(dev).cuda_stream))
-    return out, status, residual, fitness
+    return _refine_call(_lib.load().gp_icp_refine_masked,
+                        (F, H, W, C.byref(ms.c), n, det_idx.data_ptr(), rendered.data_ptr(), boxes.data_ptr(),
+                         poses.data_ptr(), K.data_ptr(), C.byref(p)), n, poses.device, torch.float32, scene_ws, scratch)
 
 
 @torch.no_grad()
@@ -345,19 +363,12 @@ def refine_icp_masked(meshes_dev, labels, poses, depth, K, det_frame, det_idx, m
     device = poses.device
     F, H, W = depth.shape
     n = poses.shape[0]
-    out = poses.clone()
-    status = torch.empty(n, dtype=torch.int32, device=device)
-    residual = torch.empty(n, device=device)
-    fitness = torch.empty(n, device=device)
+    out = _outputs(n, device, torch.float32)
     if n == 0:
-        return out, status, residual, fitness
+        return out
     ws, ms, box_pixels = masked_scene(depth, K, det_frame, masks, rle, upm)
     di = torch.as_tensor(det_idx, dtype=torch.int32).to(device)
-    chunk = max(1, min(n, WORKSPACE_BYTES // (box_pixels * 12 + 52 * H * W)))
-    for s in range(0, n, chunk):
-        sl = slice(s, min(n, s + chunk))
-        rendered, boxes = render_hypotheses(meshes_dev, labels[sl], poses[sl], K, frame_idx[sl], H, W, upm)
-        o = refine_rendered_masked(ms, ws, box_pixels, depth, K, di[sl].contiguous(), rendered, boxes, poses[sl],
-                                   **params)
-        out[sl], status[sl], residual[sl], fitness[sl] = o
-    return out, status, residual, fitness
+    return _render_and_run(meshes_dev, labels, poses, K, frame_idx, H, W, upm, box_pixels * 12,
+                           lambda sl, rendered, boxes: refine_rendered_masked(
+                               ms, ws, box_pixels, depth, K, di[sl].contiguous(), rendered, boxes, poses[sl], **params),
+                           out)

@@ -434,13 +434,15 @@ class GigaPose(LightningModule):
         (gigapose_b200.teaser.refine_teaserpp, params as gigapose_b200.teaser.DEFAULTS) and the collection carries
         `teaser_status`, `teaser_inliers` and `teaser_clique` [B,hypotheses] in place of the ICP's three; `rank` works
         the same.  The reference's TEASER++ refiner takes no masks, so `masks` and `mask_normals` are refused with it."""
-        from gigapose_b200.icp import DEFAULTS, refine_icp, refine_icp_masked, score_hypotheses
+        from gigapose_b200.icp import refine_icp_masked, score_hypotheses
+        from gigapose_b200.teaser import REFINERS
         if K is None:
             raise TypeError("refine_depth needs K=, the frames' full-image intrinsics [F,3,3] or [3,3]")
-        if refiner not in ("icp", "teaserpp"):
-            raise ValueError(f"refiner must be 'icp' or 'teaserpp', got {refiner!r}")
-        if refiner == "teaserpp" and (masks is not None or mask_normals):
-            raise ValueError("refiner='teaserpp' takes no masks: the reference's TEASER++ refiner ignores them")
+        if refiner not in REFINERS:
+            raise ValueError(f"refiner must be {' or '.join(map(repr, REFINERS))}, got {refiner!r}")
+        r = REFINERS[refiner]
+        if not r.masks and (masks is not None or mask_normals):
+            raise ValueError(f"refiner={refiner!r} takes no masks: the reference's refiner ignores them")
         meshes = self.meshes[dataset_name]
         poses = predictions.pred_poses
         B, k = poses.shape[:2]
@@ -455,36 +457,28 @@ class GigaPose(LightningModule):
             else:
                 raise ValueError("frame_idx is needed when depth holds several frames")
         frame_idx = np.asarray(torch.as_tensor(frame_idx).cpu()).reshape(-1)
-        labels = object_indices(predictions.infos, len(meshes))
-        if refiner == "teaserpp":
-            from gigapose_b200.teaser import refine_teaserpp
-            out, status, inliers, clique = refine_teaserpp(meshes, np.repeat(labels, h), poses[:, :h].reshape(-1, 4, 4),
-                                                           depth, K, np.repeat(frame_idx, h), **params)
-            extra = dict(teaser_status=status, teaser_inliers=inliers, teaser_clique=clique)
-        elif mask_normals:
+        labels = np.repeat(object_indices(predictions.infos, len(meshes)), h)
+        hyp_poses = poses[:, :h].reshape(-1, 4, 4)
+        if mask_normals:
             if masks is None:
                 raise ValueError("mask_normals=True needs masks, dense [B,H,W] or dict(counts=, offsets=)")
             dense, rle = (None, (masks["counts"], masks["offsets"])) if isinstance(masks, dict) else (masks, None)
-            out, status, residual, fitness = refine_icp_masked(
-                meshes, np.repeat(labels, h), poses[:, :h].reshape(-1, 4, 4), depth, K, frame_idx,
-                np.repeat(np.arange(B), h), dense, rle, **params)
+            out, *extra = refine_icp_masked(meshes, labels, hyp_poses, depth, K, frame_idx, np.repeat(np.arange(B), h),
+                                            dense, rle, **params)
         else:
             if masks is not None:
-                masks = torch.as_tensor(masks).to(poses.device).repeat_interleave(h, 0)
-            out, status, residual, fitness = refine_icp(meshes, np.repeat(labels, h), poses[:, :h].reshape(-1, 4, 4),
-                                                        depth, K, np.repeat(frame_idx, h), masks, **params)
-        if refiner == "icp":
-            extra = dict(icp_status=status, icp_residual=residual, icp_fitness=fitness)
+                params = dict(params, masks=torch.as_tensor(masks).to(poses.device).repeat_interleave(h, 0))
+            out, *extra = r.refine(meshes, labels, hyp_poses, depth, K, np.repeat(frame_idx, h), **params)
         refined = predictions.clone()
         refined.register_tensor("poses_input", poses.clone())
         new = poses.clone()
         new[:, :h] = out.reshape(B, h, 4, 4)
         refined.register_tensor("pred_poses", new)
-        for name, v in extra.items():
+        for name, v in zip(r.outputs, extra):
             refined.register_tensor(name, v.reshape(B, h))
         if rank:
-            counts, score, best = score_hypotheses(meshes, np.repeat(labels, h), out, depth, K, np.repeat(frame_idx, h), h,
-                                                   unit_per_m=params.get("unit_per_m", DEFAULTS["unit_per_m"]))
+            counts, score, best = score_hypotheses(meshes, labels, out, depth, K, np.repeat(frame_idx, h), h,
+                                                   unit_per_m=params.get("unit_per_m", r.defaults["unit_per_m"]))
             refined.register_tensor("depth_counts", counts.reshape(B, h, 4))
             refined.register_tensor("depth_score", score.reshape(B, h))
             refined.register_tensor("best_hypothesis", best.to(torch.int64))

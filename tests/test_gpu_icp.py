@@ -169,6 +169,53 @@ def test_deterministic_and_independent_of_the_batch():
     print("statuses of the batch of 40:", np.bincount(a[1].numpy(), minlength=6).tolist())
 
 
+def test_chunk_boundaries_change_no_output(monkeypatch):
+    """ICP with and without masks, masked ICP, TEASER++ and the depth score, with WORKSPACE_BYTES lowered so that the
+    12 hypotheses (4 detections of 3 in 2 frames) split into chunks of one hypothesis (one detection for the score)
+    and of a few: every output equals the one-chunk run's bit for bit."""
+    from gigapose_b200 import teaser
+    meshes = [ellipsoid(), assembly()]
+    dm = icp.device_meshes(meshes, DEV)
+    frames = [scene(meshes[o], T) for o, T in ((0, T_ELL), (1, T_ASM))]
+    depth, frame_masks = torch.stack([d for d, _ in frames]), torch.stack([m for _, m in frames])
+    rng = np.random.default_rng(3)
+    det_frame, n_hyp = np.array([0, 1, 1, 0]), 3
+    fidx = np.repeat(det_frame, n_hyp)
+    T0 = torch.as_tensor(np.stack([perturb((T_ELL, T_ASM)[f], rng.normal(size=3), rng.uniform(1, 8),
+                                           rng.uniform(-10, 10, 3)) for f in fidx])).to(DEV)
+    Kt = torch.as_tensor(K)
+    det_idx = np.repeat(np.arange(4), n_hyp)
+
+    stages = [lambda: icp.refine_icp(dm, fidx, T0, depth, Kt, fidx),
+              lambda: icp.refine_icp(dm, fidx, T0, depth, Kt, fidx, frame_masks[fidx]),
+              lambda: icp.refine_icp_masked(dm, fidx, T0, depth, Kt, det_frame, det_idx, masks=frame_masks[det_frame]),
+              lambda: teaser.refine_teaserpp(dm, fidx, T0, depth, Kt, fidx),
+              lambda: icp.score_hypotheses(dm, fidx, T0, depth, Kt, fidx, n_hyp)]
+    renders = []                                                       # hypotheses per chunk, each stage's
+    render_hypotheses = icp.render_hypotheses
+    monkeypatch.setattr(icp, "render_hypotheses", lambda *a: renders[-1].append(len(a[1])) or render_hypotheses(*a))
+
+    def run_all():
+        outs = []
+        renders.clear()
+        for stage in stages:
+            renders.append([])
+            outs.append([x.cpu().numpy().tobytes() for x in stage()])
+        return outs
+
+    want = run_all()
+    assert renders == [[12]] * 5
+    for budget in (1, 5 * 52 * H * W):
+        monkeypatch.setattr(icp, "WORKSPACE_BYTES", budget)
+        got = run_all()
+        print(f"WORKSPACE_BYTES {budget}: hypotheses per chunk {renders}")
+        assert all(len(r) > 1 and sum(r) == 12 for r in renders)
+        if budget == 1:
+            assert renders == [[1] * 12] * 4 + [[3] * 4]
+        for stage, (a, b) in enumerate(zip(want, got)):
+            assert a == b, stage
+
+
 def test_gigapose_refine_depth_surface(tmp_path):
     import os
     import sys
